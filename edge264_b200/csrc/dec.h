@@ -135,8 +135,9 @@ typedef struct SliceCtx {
 	MvCache mc;
 } SliceCtx;
 
-/* One slice waiting to be parsed (threaded mode): its own copy of the RBSP and a slice context prepared by the header
- * parser.  dep = the picture whose records a B slice reads as co-located motion (must be completely parsed first). */
+/* One slice waiting to be parsed: its own copy of the RBSP and of the co-located picture's slot_uid table, and a slice
+ * context prepared by the header parser.  dep = the picture whose records a B slice reads as co-located motion (must
+ * be completely parsed first). */
 struct PicBuild;
 typedef struct SliceJob {
 	struct SliceJob *next;
@@ -147,17 +148,16 @@ typedef struct SliceJob {
 	SliceCtx sc;
 } SliceJob;
 
-/* One picture between its first slice header and its submission to the backend.  The synchronous decoder has one;
- * with worker threads (edge264_alloc n_threads != 0) several pictures are parsed at the same time, like the
- * reference's slice tasks (edge264_internal.h:223-261, worker_loop edge264_headers.c:450-603). */
+/* One picture between its first slice header and its submission to the backend.  Without worker threads there is one
+ * and the calling thread does its work; with workers (edge264_alloc n_threads != 0) several pictures are parsed at
+ * the same time, like the reference's slice tasks (edge264_internal.h:223-261, worker_loop edge264_headers.c:450-603). */
 typedef struct PicBuild {
 	MbInfo *mbi;
 	E264MbRec *recs; int16_t *coefs; uint32_t coef_cap, n_coefs;
 	E264SliceRec *slices; int n_slices;
 	uint32_t *intra_list; int staging;
 	int mbs_done, n_intra, any_deblock; uint16_t slice_counter;
-	int slot, host_buf, conceal_ref, error;
-	/* threaded mode */
+	int slot, host_buf, conceal_ref;
 	int in_use, closed, running, parsed;
 	uint64_t seq;
 	E264PicDesc pd;           /* filled when parsed: what goes to the backend when the picture's turn comes */
@@ -181,7 +181,6 @@ typedef struct HostBuf {
 struct Edge264Decoder {
 	/* configuration */
 	Edge264AllocCb alloc_cb; Edge264FreeCb free_cb; void *alloc_arg;
-	Edge264LogCb log_cb; void *log_arg;
 	const struct E264Backend *be; void *be_ctx;
 	/* parameter sets */
 	SPS sps; PPS pps[E264_MAX_PPS];
@@ -191,20 +190,17 @@ struct Edge264Decoder {
 	/* DPB */
 	Pic pics[E264_MAX_SLOTS];
 	int cur;                           /* slot of the picture being decoded, -1 none */
-	int cur_is_ref, cur_idr, cur_nal_ref_idc;
-	int prev_ref_frame_num, prev_poc_msb, prev_poc_lsb, prev_frame_num_offset, prev_frame_num, prev_has_mmco5;
-	int last_idr_pic_id, last_poc_lsb, last_delta_poc0;
-	int frame_num_offset;
+	int cur_idr, cur_nal_ref_idc;
+	int prev_ref_frame_num, prev_poc_msb;
 	int q_prev_ref_frame_num, q_cur_frame_num;   /* reference-style absolute frame numbers, only used to number FrameIds like it */
 	int32_t next_uid;
-	int mmco5_seen;
 	SliceHeader sh;                    /* header of the slice being parsed */
 	SliceHeader first_sh;              /* header of the first slice of the current picture (marking) */
 	/* current picture build-up */
 	PicBuild *pb;                      /* the picture slices are being added to (NULL between pictures) */
 	PicBuild builds[E264_MAX_BUILDS];
 	int n_builds;
-	/* worker threads (0 = synchronous parsing inside edge264_decode_NAL) */
+	/* worker threads (0 = the calling thread parses and submits each picture inside edge264_decode_NAL) */
 	int n_threads, stop;
 	pthread_t threads[E264_MAX_THREADS];
 	pthread_mutex_t lock, be_lock;     /* lock: builds, queues, hb[].submitted; be_lock: backend calls from several threads */
@@ -219,9 +215,8 @@ struct Edge264Decoder {
 	int pending_release;               /* host buffer handed out without borrow, released at next decode_NAL */
 	int sync_output;                   /* E264_SYNC_OUTPUT=1: get_frame always waits for the device (the behaviour before round 2's last step; A/B switch) */
 	int block_output;                  /* the last decode_NAL asked the application to fetch frames (ENOBUFS, end of stream): get_frame waits for the device */
-	/* scratch */
+	/* scratch: RBSP of the last non-slice NAL unit */
 	uint8_t *rbsp; size_t rbsp_cap;
-	SliceCtx sc;
 };
 
 /* backend = the thing that turns records into pixels.  The product library binds the CUDA

@@ -16,8 +16,6 @@
 #include "dec.h"
 #include "h264_tables.h"
 
-int e264_parse_slice_data(SliceCtx *s);   /* slice_dec.c */
-
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
 static int prof_on = -1;
@@ -245,9 +243,9 @@ static int hostbuf_acquire(Edge264Decoder *d) {
 			if (!smp) return -1;
 			d->hb[i].p = (uint8_t *)smp; d->hb[i].mbs = mbs;
 		} else {
-			if (d->n_threads) pthread_mutex_lock(&d->be_lock);
+			pthread_mutex_lock(&d->be_lock);
 			d->hb[i].p = (uint8_t *)d->be->host_alloc(d->be_ctx, bytes);
-			if (d->n_threads) pthread_mutex_unlock(&d->be_lock);
+			pthread_mutex_unlock(&d->be_lock);
 			if (!d->hb[i].p) return -1;
 		}
 		return i;
@@ -295,7 +293,7 @@ static int bump_frame(Edge264Decoder *d, int ignore_slot) {
 	p->needed_for_output = 0;
 	if (p->host_buf >= 0) {
 		d->hb[p->host_buf].state = 2; d->outq[d->outq_n++] = p->host_buf;
-		if (d->hb[p->host_buf].submitted) p->host_buf = -1;
+		if (__atomic_load_n(&d->hb[p->host_buf].submitted, __ATOMIC_ACQUIRE)) p->host_buf = -1;   /* a worker may be submitting it */
 	}
 	slot_release_if_unused(d, best);
 	return 1;
@@ -343,8 +341,8 @@ static int conceal_reference(Edge264Decoder *d) {
 }
 
 /* data side of a finished picture: conceal what no slice delivered and list the intra macroblocks (build_finalize: the
- * records are complete afterwards), then hand the picture to the backend (build_submit).  Both run in the calling
- * thread (synchronous mode) or in a worker once every slice is parsed. */
+ * records are complete afterwards), then hand the picture to the backend (build_submit).  build_work runs both once
+ * the picture is closed and every slice of it is parsed. */
 static void build_finalize(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd) {
 	if (pb->mbs_done < d->w_mbs * d->h_mbs) conceal_missing(d, pb);
 	memset(pd, 0, sizeof(*pd));
@@ -364,24 +362,20 @@ static int build_submit(Edge264Decoder *d, PicBuild *pb, const E264PicDesc *pd, 
 	return r ? EIO : 0;
 }
 
-static void close_picture_threaded(Edge264Decoder *d);
+static int build_work(Edge264Decoder *d, PicBuild *pb);
 
+/* Close the current picture: no later slice joins it.  With workers, one of them finalizes and submits it; with none,
+ * the calling thread does it here and the backend's error is returned. */
 static int finish_picture(Edge264Decoder *d) {
 	if (d->cur < 0) return 0;
 	Pic *p = &d->pics[d->cur];
 	int ret = 0;
-	if (d->n_threads) close_picture_threaded(d);
-	else {
-		PicBuild *pb = d->pb;
-		pb->conceal_ref = conceal_reference(d);
-		if (p->host_buf >= 0) {
-			uint64_t ticket = 0; E264PicDesc pd;
-			build_finalize(d, pb, &pd);
-			ret = build_submit(d, pb, &pd, &ticket);
-			d->hb[p->host_buf].ticket = ticket; __atomic_store_n(&d->hb[p->host_buf].submitted, 1, __ATOMIC_RELEASE);
-		}
-		pb->in_use = 0;
-	}
+	pthread_mutex_lock(&d->lock);
+	d->pb->conceal_ref = conceal_reference(d);
+	d->pb->closed = 1;
+	pthread_cond_broadcast(&d->work_cv);
+	if (!d->n_threads) ret = build_work(d, d->pb);
+	pthread_mutex_unlock(&d->lock);
 	d->pb = NULL;
 	if (p->host_buf >= 0 && !p->needed_for_output) p->host_buf = -1;   /* already in the output queue */
 	apply_marking(d);
@@ -392,22 +386,24 @@ static int finish_picture(Edge264Decoder *d) {
 }
 
 /* ------------------------------------------------------------------------------------------ */
-/* worker threads: several pictures parsed at the same time                                      */
+/* picture pipeline: slices queued on builds, parsed and submitted by build_work                  */
 /* ------------------------------------------------------------------------------------------ */
-/* The calling thread parses headers, runs the decoded-picture-buffer logic and queues slices; workers parse slice
- * data.  One worker owns a picture at a time (its slices share the coefficient pool and run in order); pictures are
- * handed to the backend strictly in decoding order.  A B slice waits until its co-located picture is completely
- * parsed (its records are the motion data direct prediction reads); nothing else depends on another picture at parse
- * time — pixels are the device's business.  Reference counterpart: task dependencies + worker_loop,
- * edge264_internal.h:1196-1226, edge264_headers.c:450-603. */
+/* The calling thread parses headers, runs the decoded-picture-buffer logic and queues slices; build_work parses slice
+ * data.  Worker threads run it, several pictures at a time; with no workers the calling thread runs it as soon as a
+ * slice is queued and when the picture is closed, so every picture is submitted before the next one starts.  One thread
+ * owns a picture at a time (its slices share the coefficient pool and run in order); pictures are handed to the backend
+ * strictly in decoding order.  A B slice waits until its co-located picture is completely parsed (its records are the
+ * motion data direct prediction reads); nothing else depends on another picture at parse time — pixels are the
+ * device's business.  Reference counterpart: task dependencies + worker_loop, edge264_internal.h:1196-1226,
+ * edge264_headers.c:450-603. */
 static PicBuild *build_acquire(Edge264Decoder *d, int slot) {
-	if (!d->n_threads) { PicBuild *pb = &d->builds[0]; pb->in_use = 1; return pb; }
 	pthread_mutex_lock(&d->lock);
 	PicBuild *pb = NULL;
 	for (;;) {
 		/* the slot's records may still be written by its previous picture's parser or read as co-located motion */
 		if (d->slot_users[slot] == 0) for (int i = 0; i < d->n_builds && !pb; i++) if (!d->builds[i].in_use) pb = &d->builds[i];
 		if (pb) break;
+		/* not reached without workers: every earlier picture has been submitted, which frees its build and its slots */
 		pthread_cond_wait(&d->done_cv, &d->lock);
 	}
 	MbInfo *mbi = pb->mbi;
@@ -429,26 +425,68 @@ static void slice_enqueue(Edge264Decoder *d, PicBuild *pb, SliceJob *job, int co
 	pthread_cond_broadcast(&d->work_cv);
 	pthread_mutex_unlock(&d->lock);
 }
-static void close_picture_threaded(Edge264Decoder *d) {
-	pthread_mutex_lock(&d->lock);
-	d->pb->conceal_ref = conceal_reference(d);
-	d->pb->closed = 1;
-	pthread_cond_broadcast(&d->work_cv);
-	pthread_mutex_unlock(&d->lock);
-}
 /* wait until every picture has been parsed and handed to the backend (flush, end of stream, format change) */
 static void threads_drain(Edge264Decoder *d) {
-	if (!d->n_threads) return;
 	pthread_mutex_lock(&d->lock);
 	for (;;) {
 		int busy = 0;
 		for (int i = 0; i < d->n_builds; i++) busy |= d->builds[i].in_use;
 		if (!busy) break;
+		/* not reached without workers: the picture under construction, if any, was closed before, which submitted it */
 		pthread_cond_wait(&d->done_cv, &d->lock);
 	}
 	pthread_mutex_unlock(&d->lock);
 }
 static inline int job_ready(const SliceJob *j) { return !j->dep || j->dep->seq != j->dep_seq || j->dep->parsed || !j->dep->in_use; }
+/* The work of one build, called with d->lock held: parse its queued slices while they are ready; once the picture is
+ * closed and completely parsed, finalize it and hand the parsed pictures to the backend in decoding order.  Returns
+ * the first slice-data error (EBADMSG, ENOMEM when the coefficient pool runs out) or the backend's EIO. */
+static int build_work(Edge264Decoder *d, PicBuild *pb) {
+	int ret = 0;
+	pb->running = 1;
+	while (pb->head && job_ready(pb->head)) {
+		SliceJob *job = pb->head;
+		pb->head = job->next; if (!pb->head) pb->tail = NULL;
+		pthread_mutex_unlock(&d->lock);
+		job->sc.n_coefs = pb->n_coefs;      /* the slices of a picture share one coefficient pool */
+		int n = e264_parse_slice_data(&job->sc);
+		pb->n_coefs = job->sc.n_coefs; pb->n_intra += job->sc.n_intra;
+		if (n > 0) pb->mbs_done += n;
+		if (job->sc.error && !ret) ret = job->sc.error == 2 ? ENOMEM : EBADMSG;
+		free(job->rbsp);
+		pthread_mutex_lock(&d->lock);
+		if (job->col_slot >= 0) { d->slot_users[job->col_slot]--; pthread_cond_broadcast(&d->done_cv); }
+		free(job);
+	}
+	if (!pb->head && pb->closed) {
+		pthread_mutex_unlock(&d->lock);
+		build_finalize(d, pb, &pb->pd);
+		pthread_mutex_lock(&d->lock);
+		pb->parsed = 1; pb->running = 0;      /* its records are complete: B pictures may read them */
+		pthread_cond_broadcast(&d->work_cv);
+		/* hand parsed pictures to the backend in decoding order; whoever completes the oldest one also sends the
+		 * ones that were waiting behind it, so no worker ever sleeps on the order */
+		while (!d->submitting) {
+			PicBuild *q = NULL;
+			for (int i = 0; i < d->n_builds; i++) if (d->builds[i].in_use && d->builds[i].parsed && d->builds[i].seq == d->submit_seq) q = &d->builds[i];
+			if (!q) break;
+			uint64_t ticket = 0;
+			d->submitting = 1;
+			pthread_mutex_unlock(&d->lock);
+			pthread_mutex_lock(&d->be_lock);
+			int r = build_submit(d, q, &q->pd, &ticket);
+			pthread_mutex_unlock(&d->be_lock);
+			if (r && !ret) ret = r;
+			pthread_mutex_lock(&d->lock);
+			if (q->host_buf >= 0) { d->hb[q->host_buf].ticket = ticket; __atomic_store_n(&d->hb[q->host_buf].submitted, 1, __ATOMIC_RELEASE); }
+			d->submit_seq++; d->submitting = 0;
+			d->slot_users[q->slot]--;
+			q->in_use = 0;
+			pthread_cond_broadcast(&d->done_cv);
+		}
+	} else pb->running = 0;               /* more slices to come, or the next one waits for its co-located picture */
+	return ret;
+}
 static void *worker_main(void *arg) {
 	Edge264Decoder *d = (Edge264Decoder *)arg;
 	pthread_mutex_lock(&d->lock);
@@ -465,53 +503,12 @@ static void *worker_main(void *arg) {
 			pthread_cond_wait(&d->work_cv, &d->lock);
 		}
 		if (d->stop) break;
-		pb->running = 1;
-		while (pb->head && job_ready(pb->head)) {
-			SliceJob *job = pb->head;
-			pb->head = job->next; if (!pb->head) pb->tail = NULL;
-			pthread_mutex_unlock(&d->lock);
-			job->sc.n_coefs = pb->n_coefs;      /* the slices of a picture share one coefficient pool */
-			int n = e264_parse_slice_data(&job->sc);
-			pb->n_coefs = job->sc.n_coefs; pb->n_intra += job->sc.n_intra;
-			if (n > 0) pb->mbs_done += n;
-			if (job->sc.error) pb->error = job->sc.error;
-			free(job->rbsp);
-			pthread_mutex_lock(&d->lock);
-			if (job->col_slot >= 0) { d->slot_users[job->col_slot]--; pthread_cond_broadcast(&d->done_cv); }
-			free(job);
-		}
-		if (!pb->head && pb->closed) {
-			pthread_mutex_unlock(&d->lock);
-			build_finalize(d, pb, &pb->pd);
-			pthread_mutex_lock(&d->lock);
-			pb->parsed = 1; pb->running = 0;      /* its records are complete: B pictures may read them */
-			pthread_cond_broadcast(&d->work_cv);
-			/* hand parsed pictures to the backend in decoding order; whoever completes the oldest one also sends the
-			 * ones that were waiting behind it, so no worker ever sleeps on the order */
-			while (!d->submitting) {
-				PicBuild *q = NULL;
-				for (int i = 0; i < d->n_builds; i++) if (d->builds[i].in_use && d->builds[i].parsed && d->builds[i].seq == d->submit_seq) q = &d->builds[i];
-				if (!q) break;
-				uint64_t ticket = 0;
-				d->submitting = 1;
-				pthread_mutex_unlock(&d->lock);
-				pthread_mutex_lock(&d->be_lock);
-				build_submit(d, q, &q->pd, &ticket);
-				pthread_mutex_unlock(&d->be_lock);
-				pthread_mutex_lock(&d->lock);
-				if (q->host_buf >= 0) { d->hb[q->host_buf].ticket = ticket; __atomic_store_n(&d->hb[q->host_buf].submitted, 1, __ATOMIC_RELEASE); }
-				d->submit_seq++; d->submitting = 0;
-				d->slot_users[q->slot]--;
-				q->in_use = 0;
-				pthread_cond_broadcast(&d->done_cv);
-			}
-		} else pb->running = 0;               /* more slices to come, or the next one waits for its co-located picture */
+		build_work(d, pb);
 	}
 	pthread_mutex_unlock(&d->lock);
 	return NULL;
 }
 static void threads_stop(Edge264Decoder *d) {
-	if (!d->n_threads) return;
 	threads_drain(d);
 	pthread_mutex_lock(&d->lock);
 	d->stop = 1;
@@ -592,10 +589,10 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	d->stride_c = w; if (!(d->stride_c & 4095)) d->stride_c += 16;       /* headers.c:2035-2037 pads by 8; 16 keeps both chroma planes 8-byte aligned for vector stores and TMA */
 	d->plane_y = d->stride_y * h; d->plane_c = d->stride_c * (h >> 1);
 	d->frame_bytes = d->plane_y + d->plane_c + 16;
-	if (d->n_threads) pthread_mutex_lock(&d->lock);      /* idle workers scan builds[0..n_builds) */
+	pthread_mutex_lock(&d->lock);      /* idle workers scan builds[0..n_builds) */
 	d->n_builds = d->n_threads ? d->n_threads + 2 : 1;
 	if (d->n_builds > E264_MAX_BUILDS) d->n_builds = E264_MAX_BUILDS;
-	if (d->n_threads) pthread_mutex_unlock(&d->lock);
+	pthread_mutex_unlock(&d->lock);
 	/* a picture keeps its slot (and the slot's record buffer) until it is handed to the device: parsing ahead needs one spare slot per picture in flight */
 	d->n_slots = s->max_num_ref_frames + 2 + (d->n_threads ? d->n_builds : 0);
 	if (d->n_slots > E264_MAX_SLOTS) d->n_slots = E264_MAX_SLOTS;
@@ -605,14 +602,14 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	hostbufs_free_all(d);
 	if (d->be->configure(d->be_ctx, &g, d->n_slots)) return ENOMEM;
 	int oom = 0;
-	if (d->n_threads) pthread_mutex_lock(&d->lock);
+	pthread_mutex_lock(&d->lock);
 	for (int i = 0; i < E264_MAX_BUILDS; i++) {
 		free(d->builds[i].mbi); memset(&d->builds[i], 0, sizeof(d->builds[i]));
 		if (i < d->n_builds && !(d->builds[i].mbi = (MbInfo *)calloc((size_t)d->w_mbs * d->h_mbs, sizeof(MbInfo)))) oom = 1;
 	}
 	d->pb = NULL;
 	memset(d->slot_users, 0, sizeof(d->slot_users)); memset(d->slot_build, 0, sizeof(d->slot_build));
-	if (d->n_threads) pthread_mutex_unlock(&d->lock);
+	pthread_mutex_unlock(&d->lock);
 	if (oom) return ENOMEM;
 	memset(d->pics, 0, sizeof(d->pics));
 	for (int i = 0; i < E264_MAX_SLOTS; i++) d->pics[i].host_buf = -1;
@@ -626,7 +623,7 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	o->frame_crop_offsets[0] = (int16_t)s->crop[2]; o->frame_crop_offsets[1] = (int16_t)s->crop[1];
 	o->frame_crop_offsets[2] = (int16_t)s->crop[3]; o->frame_crop_offsets[3] = (int16_t)s->crop[0];
 	d->configured = 1;
-	if (!keep_numbering) { d->q_prev_ref_frame_num = -1; d->prev_ref_frame_num = -1; d->prev_poc_msb = d->prev_poc_lsb = 0; }
+	if (!keep_numbering) { d->q_prev_ref_frame_num = -1; d->prev_ref_frame_num = -1; d->prev_poc_msb = 0; }
 	return 0;
 }
 
@@ -787,22 +784,20 @@ static void build_ref_lists(Edge264Decoder *d, const SliceHeader *h, int lists[2
 /* ------------------------------------------------------------------------------------------ */
 /* slice NAL                                                                                    */
 /* ------------------------------------------------------------------------------------------ */
+/* the first free slot, preferring one no parser is still using: taking a busy one would wait in build_acquire for its
+ * picture to be submitted (without workers no slot is busy here, so this is the first free slot) */
 static int find_free_slot(Edge264Decoder *d) {
-	if (d->n_threads) {   /* prefer a slot no parser is still using: taking a busy one would wait for its picture to be submitted */
-		int pick = -1;
-		pthread_mutex_lock(&d->lock);
-		for (int i = 0; i < d->n_slots && pick < 0; i++) if (!d->pics[i].in_use && d->slot_users[i] == 0) pick = i;
-		pthread_mutex_unlock(&d->lock);
-		if (pick >= 0) return pick;
-	}
-	for (int i = 0; i < d->n_slots; i++) if (!d->pics[i].in_use) return i;
-	return -1;
+	int pick = -1;
+	pthread_mutex_lock(&d->lock);
+	for (int i = 0; i < d->n_slots && pick < 0; i++) if (!d->pics[i].in_use && d->slot_users[i] == 0) pick = i;
+	for (int i = 0; i < d->n_slots && pick < 0; i++) if (!d->pics[i].in_use) pick = i;
+	pthread_mutex_unlock(&d->lock);
+	return pick;
 }
 
-static PicBuild *build_acquire(Edge264Decoder *d, int slot);
-static void slice_enqueue(Edge264Decoder *d, PicBuild *pb, SliceJob *job, int col_slot);
-
-static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, BitReader *b, SliceJob *job) {
+/* Parses the slice header, starts a picture when it is the first slice of one and queues the slice's data on the
+ * picture's build.  *jobp is set to NULL once the job is queued; until then it stays the caller's. */
+static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, BitReader *b, SliceJob **jobp) {
 	SliceHeader *h = &d->sh;
 	const PPS *p = NULL;
 	int ret = parse_slice_header(d, b, nal_unit_type, nal_ref_idc, h, &p);
@@ -822,11 +817,11 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 
 	if (d->cur < 0) {
 		if (d->outq_n > 16) {
-			if (d->n_threads) {   /* the frame the application is told to fetch may still be with a parser: wait for it here, not in a polling loop */
-				pthread_mutex_lock(&d->lock);
-				while (!__atomic_load_n(&d->hb[d->outq[0]].submitted, __ATOMIC_ACQUIRE)) pthread_cond_wait(&d->done_cv, &d->lock);
-				pthread_mutex_unlock(&d->lock);
-			}
+			/* the frame the application is told to fetch may still be with a parser: wait for it here, not in a polling
+			 * loop (without workers every queued frame has been submitted, so this does not wait) */
+			pthread_mutex_lock(&d->lock);
+			while (!__atomic_load_n(&d->hb[d->outq[0]].submitted, __ATOMIC_ACQUIRE)) pthread_cond_wait(&d->done_cv, &d->lock);
+			pthread_mutex_unlock(&d->lock);
 			return ENOBUFS;
 		}
 		int hbuf = hostbuf_acquire(d);
@@ -834,7 +829,7 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 		/* frame_num and POC (8.2.1), with absolute (unwrapped) frame numbers like the reference (headers.c:1059) */
 		int prev = d->prev_ref_frame_num;
 		int frame_num_abs = idr ? 0 : prev + 1 + ((h->frame_num - prev - 1) & mask);
-		if (idr) { d->prev_ref_frame_num = -1; d->prev_poc_msb = d->prev_poc_lsb = 0; }
+		if (idr) { d->prev_ref_frame_num = -1; d->prev_poc_msb = 0; }
 		int poc, poc_top;
 		if (s->poc_type == 0) {
 			int sh = 32 - s->log2_max_poc_lsb;
@@ -889,7 +884,7 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 				}
 				np->poc = np->poc_dec = np->poc_top = np->poc_top_dec = npoc;
 				for (int i = 0; i < E264_MAX_SLOTS; i++) np->slot_uid[i] = -1;
-				if (d->be->fill_slot) { if (d->n_threads) pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, 0); if (d->n_threads) pthread_mutex_unlock(&d->be_lock); }
+				if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, 0); pthread_mutex_unlock(&d->be_lock); }
 			}
 			d->prev_ref_frame_num = frame_num_abs - 1;   /* the last inserted frame is the previous reference frame now (headers.c:1131) */
 		}
@@ -921,19 +916,18 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 		d->cur = slot; d->cur_idr = idr; d->cur_nal_ref_idc = nal_ref_idc;
 		d->first_sh = *h;
 		for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = d->pics[i].in_use ? d->pics[i].uid : -1;
-		PicBuild *pb = build_acquire(d, slot);     /* threaded mode: may wait for a parser to finish */
+		PicBuild *pb = build_acquire(d, slot);     /* may wait for a worker to finish a picture */
 		E264Staging stg; memset(&stg, 0, sizeof(stg));
 		int ar;
-		{ PROF_BEGIN; if (d->n_threads) pthread_mutex_lock(&d->be_lock); ar = d->be->acquire_staging(d->be_ctx, slot, &stg); if (d->n_threads) pthread_mutex_unlock(&d->be_lock); PROF_END(1); }
+		{ PROF_BEGIN; pthread_mutex_lock(&d->be_lock); ar = d->be->acquire_staging(d->be_ctx, slot, &stg); pthread_mutex_unlock(&d->be_lock); PROF_END(1); }
 		if (ar) {   /* give the build back as if it had never been taken (no later picture exists yet) */
-			if (d->n_threads) { pthread_mutex_lock(&d->lock); d->next_seq--; d->slot_users[slot]--; d->slot_build[slot] = NULL; pb->in_use = 0; pthread_mutex_unlock(&d->lock); }
-			else pb->in_use = 0;
+			pthread_mutex_lock(&d->lock); d->next_seq--; d->slot_users[slot]--; d->slot_build[slot] = NULL; pb->in_use = 0; pthread_mutex_unlock(&d->lock);
 			cp->in_use = 0; d->cur = -1; d->hb[hbuf].state = 0;
 			return ENOMEM;
 		}
 		cp->recs = stg.recs;
 		pb->recs = stg.recs; pb->coefs = stg.coefs; pb->slices = stg.slices; pb->intra_list = stg.intra_list; pb->staging = stg.handle;
-		pb->coef_cap = stg.coef_capacity; pb->n_coefs = 0; pb->n_slices = 0; pb->mbs_done = 0; pb->n_intra = 0; pb->any_deblock = 0; pb->error = 0;
+		pb->coef_cap = stg.coef_capacity; pb->n_coefs = 0; pb->n_slices = 0; pb->mbs_done = 0; pb->n_intra = 0; pb->any_deblock = 0;
 		pb->slot = slot; pb->host_buf = hbuf; pb->conceal_ref = -1; pb->slice_counter = 0;
 		{ PROF_BEGIN; memset(pb->mbi, 0, (size_t)d->w_mbs * d->h_mbs * sizeof(MbInfo)); PROF_END(4); }
 		/* records need no clearing: every macroblock of a complete picture rewrites its own (sx_one_mb) */
@@ -976,7 +970,8 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 	sr->deblock_idc = (uint8_t)h->deblock_idc; sr->slice_type = (uint8_t)h->slice_type;
 	merge_scaling(s, p, sr);
 
-	SliceCtx *c = job ? &job->sc : &d->sc;
+	SliceJob *job = *jobp;
+	SliceCtx *c = &job->sc;
 	int col_slot = -1;
 	c->cabac = p->entropy_coding_mode;
 	c->w_mbs = d->w_mbs; c->h_mbs = d->h_mbs;
@@ -985,7 +980,7 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 	c->direct_spatial = h->direct_spatial; c->direct_8x8_inference = s->direct_8x8_inference; c->transform_8x8_mode = p->transform_8x8_mode;
 	c->qp = h->slice_qp; c->chroma_qp_offset[0] = p->chroma_qp_index_offset[0]; c->chroma_qp_offset[1] = p->chroma_qp_index_offset[1];
 	c->deblock_idc = h->deblock_idc; c->cur_poc = cp->poc_dec;
-	c->mbi = pb->mbi; c->recs = pb->recs; c->coefs = pb->coefs; c->n_coefs = job ? 0 : pb->n_coefs; c->coef_cap = pb->coef_cap;   /* threaded: the worker continues the pool where the previous slice ended */
+	c->mbi = pb->mbi; c->recs = pb->recs; c->coefs = pb->coefs; c->coef_cap = pb->coef_cap;   /* n_coefs: build_work continues the pool where the previous slice ended */
 	c->col_recs = NULL; c->col_slot_uid = NULL; c->error = 0; c->n_intra = 0;
 	memset(c->ref_slot, -1, sizeof(c->ref_slot)); memset(c->ref_long, 0, sizeof(c->ref_long));
 	for (int l = 0; l < 2; l++) for (int i = 0; i < 32; i++) { c->ref_uid[l][i] = -1; c->ref_poc[l][i] = 0; }
@@ -998,11 +993,10 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 			c->ref_slot[l][i] = (int8_t)sl; c->ref_uid[l][i] = d->pics[sl].uid; c->ref_poc[l][i] = d->pics[sl].poc; c->ref_long[l][i] = d->pics[sl].ref == 2;
 		}
 		if (h->slice_type == 1 && lists[1][0] >= 0) {
-			c->col_recs = d->pics[lists[1][0]].recs; c->col_slot_uid = d->pics[lists[1][0]].slot_uid;
+			c->col_recs = d->pics[lists[1][0]].recs;
 			if (d->pics[lists[1][0]].nonexisting) c->col_recs = NULL; else col_slot = lists[1][0];
-			if (job) {   /* the co-located picture's Pic entry may be recycled before this slice is parsed: keep a private copy of the uid table */
-				memcpy(job->col_slot_uid, d->pics[lists[1][0]].slot_uid, sizeof(job->col_slot_uid)); c->col_slot_uid = job->col_slot_uid;
-			}
+			/* the co-located picture's Pic entry may be recycled before this slice is parsed: keep a private copy of the uid table */
+			memcpy(job->col_slot_uid, d->pics[lists[1][0]].slot_uid, sizeof(job->col_slot_uid)); c->col_slot_uid = job->col_slot_uid;
 		}
 		int wp = h->slice_type == 0 ? p->weighted_pred_flag : p->weighted_bipred_idc;
 		sr->wp_mode = (uint8_t)wp; sr->luma_log2_wd = (uint8_t)h->luma_log2_wd; sr->chroma_log2_wd = (uint8_t)h->chroma_log2_wd;
@@ -1033,14 +1027,13 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 	c->br = *b;
 	c->mbaddr = h->first_mb;
 	c->cabac_init_idc_col = h->slice_type == 2 ? 0 : 1 + h->cabac_init_idc;
-	if (job) {   /* threaded mode: a worker parses the slice data; the picture is closed by the next picture's first slice or a flush */
-		slice_enqueue(d, pb, job, col_slot);
-		return 0;
-	}
-	int n; { PROF_BEGIN; n = e264_parse_slice_data(c); PROF_END(0); }
-	pb->n_coefs = c->n_coefs; pb->n_intra += c->n_intra;
-	if (n > 0) pb->mbs_done += n;
-	if (c->error) ret = c->error == 2 ? ENOMEM : EBADMSG;
+	slice_enqueue(d, pb, job, col_slot);
+	*jobp = NULL;
+	/* With workers, one of them parses the slice data and errors in it are not reported; the picture is closed by the
+	 * next picture's first slice, a flush, the end of the sequence or of the stream.  Without workers, the slice is
+	 * parsed here, its error is returned, and the picture is closed and submitted as soon as it is complete. */
+	if (d->n_threads) return 0;
+	{ PROF_BEGIN; pthread_mutex_lock(&d->lock); ret = build_work(d, pb); pthread_mutex_unlock(&d->lock); PROF_END(0); }
 	if (pb->mbs_done >= total) { int r2 = finish_picture(d); if (!ret) ret = r2; }
 	return ret;
 }
@@ -1056,34 +1049,33 @@ Edge264Decoder *edge264_alloc(int n_threads, Edge264LogCb log_cb, void *log_arg,
 	Edge264Decoder *d = (Edge264Decoder *)calloc(1, sizeof(*d));
 	if (!d) return NULL;
 	d->alloc_cb = (alloc_cb && free_cb) ? alloc_cb : NULL; d->free_cb = free_cb; d->alloc_arg = alloc_arg;
-	d->log_cb = log_cb; d->log_arg = log_arg;
 	d->cur = -1; d->pending_release = -1; d->prev_ref_frame_num = -1; d->q_prev_ref_frame_num = -1;
 	d->be = e264_default_backend();
 	if (!d->be || d->be->create(&d->be_ctx)) { free(d); return NULL; }
 	d->n_builds = 1;
+	pthread_mutex_init(&d->lock, NULL); pthread_mutex_init(&d->be_lock, NULL);
+	pthread_cond_init(&d->work_cv, NULL); pthread_cond_init(&d->done_cv, NULL);
 	/* n_threads as in the reference (edge264.c:223-257): 0 = parse inside edge264_decode_NAL, < 0 = one worker per CPU up
 	 * to the limit, > 0 = that many workers (here they parse slice data ahead; reconstruction is the device's) */
 	{ const char *e = getenv("E264_SYNC_OUTPUT"); d->sync_output = e && atoi(e) != 0; d->block_output = d->sync_output; }
 	if (n_threads < 0) { long n = sysconf(_SC_NPROCESSORS_ONLN); n_threads = n < 1 ? 1 : (int)n; }
 	if (n_threads > E264_MAX_THREADS) n_threads = E264_MAX_THREADS;
-	if (n_threads > 0) {
-		pthread_mutex_init(&d->lock, NULL); pthread_mutex_init(&d->be_lock, NULL);
-		pthread_cond_init(&d->work_cv, NULL); pthread_cond_init(&d->done_cv, NULL);
-		d->n_threads = n_threads;
-		for (int i = 0; i < n_threads; i++) if (pthread_create(&d->threads[i], NULL, worker_main, d)) { d->n_threads = i; threads_stop(d); d->be->destroy(d->be_ctx); free(d); return NULL; }
+	for (int i = 0; i < n_threads; i++) {
+		if (pthread_create(&d->threads[i], NULL, worker_main, d)) { edge264_free(&d); return NULL; }
+		d->n_threads = i + 1;
 	}
 	return d;
 }
 
 void edge264_flush(Edge264Decoder *d) {
 	if (!d) return;
-	if (d->cur >= 0 && d->n_threads) finish_picture(d);
+	finish_picture(d);
 	threads_drain(d);
 	/* drop every picture and the sequence state, keep parameter sets (reference edge264.c:261-270 clears them too) */
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { d->pics[i].in_use = 0; d->pics[i].host_buf = -1; }
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state != 3 || !d->hb[i].borrowed) d->hb[i].state = 0;
 	d->outq_n = 0; d->cur = -1; d->pending_release = -1;
-	d->prev_ref_frame_num = -1; d->q_prev_ref_frame_num = -1; d->prev_poc_msb = d->prev_poc_lsb = 0;
+	d->prev_ref_frame_num = -1; d->q_prev_ref_frame_num = -1; d->prev_poc_msb = 0;
 	memset(&d->sps, 0, sizeof(d->sps)); memset(d->pps, 0, sizeof(d->pps));
 	d->configured = 0;
 }
@@ -1093,10 +1085,13 @@ void edge264_free(Edge264Decoder **pd) {
 	if (!pd || !(d = *pd)) return;
 	*pd = NULL;
 	if (prof_on > 0) { for (int i = 0; i < 6; i++) if (prof_n[i]) fprintf(stderr, "host profile: %-18s %8.3f ms total %6ld calls %8.1f us/call\n", prof_names[i], 1e3 * prof_t[i], prof_n[i], 1e6 * prof_t[i] / prof_n[i]); memset(prof_t, 0, sizeof(prof_t)); memset(prof_n, 0, sizeof(prof_n)); }
-	if (d->n_threads) { if (d->cur >= 0) finish_picture(d); threads_stop(d); }
+	finish_picture(d);
+	threads_stop(d);
 	hostbufs_free_all(d);
 	d->be->destroy(d->be_ctx);
 	for (int i = 0; i < E264_MAX_BUILDS; i++) free(d->builds[i].mbi);
+	pthread_mutex_destroy(&d->lock); pthread_mutex_destroy(&d->be_lock);
+	pthread_cond_destroy(&d->work_cv); pthread_cond_destroy(&d->done_cv);
 	free(d->rbsp); free(d);
 }
 
@@ -1115,17 +1110,18 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 	}
 	int nal_ref_idc = buf[0] >> 5, nal_unit_type = buf[0] & 31;
 	size_t n = (size_t)(end - buf) - 1;
-	if (d->n_threads && (nal_unit_type == 1 || nal_unit_type == 5)) {   /* the slice is parsed later, from its own copy of the payload */
+	if (nal_unit_type == 1 || nal_unit_type == 5) {   /* the slice data is parsed from its own copy of the payload, possibly later */
 		SliceJob *job = (SliceJob *)calloc(1, sizeof(SliceJob));
-		uint8_t *rb = job ? (uint8_t *)malloc(n + 64) : NULL;
+		/* slack: the slice parsers test for an overrun once per macroblock, so a damaged slice reads past its end */
+		uint8_t *rb = job ? (uint8_t *)malloc(n + 4096) : NULL;
 		if (!rb) { free(job); return ENOMEM; }
 		size_t rn = e264_unescape(rb, buf + 1, n);
 		memset(rb + rn, 0, 32);
 		job->rbsp = rb;
 		BitReader b; br_init(&b, rb, rn);
-		int ret = decode_slice(d, nal_unit_type, nal_ref_idc, &b, job);
-		if (ret) { free(rb); free(job); }      /* not queued */
-		else if (unref_cb) unref_cb(0, unref_arg);
+		int ret = decode_slice(d, nal_unit_type, nal_ref_idc, &b, &job);
+		if (job) { free(rb); free(job); }      /* not queued */
+		if (ret == 0 && unref_cb) unref_cb(0, unref_arg);
 		return ret;
 	}
 	if (d->rbsp_cap < n + 64) { free(d->rbsp); d->rbsp_cap = n * 2 + 4096; d->rbsp = (uint8_t *)malloc(d->rbsp_cap); if (!d->rbsp) { d->rbsp_cap = 0; return ENOMEM; } }
@@ -1134,10 +1130,6 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 	BitReader b; br_init(&b, d->rbsp, rn);
 	int ret;
 	switch (nal_unit_type) {
-	case 1: case 5:
-		ret = decode_slice(d, nal_unit_type, nal_ref_idc, &b, NULL);
-		if (ret == 0 && unref_cb) unref_cb(0, unref_arg);   /* parsing is synchronous: the NAL bytes are no longer needed */
-		return ret;
 	case 7: {
 		SPS s; ret = parse_sps(d, &b, &s);
 		if (ret == 0) {
