@@ -21,7 +21,7 @@ VARIANTS := w4 w8 timing iw4 iw8
 variants: $(foreach v,$(VARIANTS),edge264_b200/variants/$(v)/libedge264_b200.so)
 edge264_b200/variants/w8/libedge264_b200.so: VFLAGS := -DINTER_WARPS=8
 edge264_b200/variants/w4/libedge264_b200.so: VFLAGS := -DINTER_WARPS=4
-edge264_b200/variants/timing/libedge264_b200.so: VFLAGS := -DE264_ROWS_TIMING
+edge264_b200/variants/timing/libedge264_b200.so: VFLAGS := -DE264_PHASE_TIMING
 edge264_b200/variants/iw4/libedge264_b200.so: VFLAGS := -DINTRA_WARPS=4
 edge264_b200/variants/iw8/libedge264_b200.so: VFLAGS := -DINTRA_WARPS=8
 edge264_b200/variants/%/libedge264_b200.so: $(CSRC)/recon.cu $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) $(CSRC)/decoder.o $(CSRC)/slice_dec.o

@@ -33,52 +33,54 @@ struct __align__(16) E264DbkMb {
 
 __device__ __forceinline__ int dbk_iabs(int v) { return v < 0 ? -v : v; }
 
-__device__ int dbk_bs_pair(const E264MbRec *p, int bp, const E264MbRec *q, int bq, bool mb_edge) {
-	if (p->kind != MBK_INTER || q->kind != MBK_INTER) return mb_edge ? 4 : 3;
-	if (((p->coded >> bp) & 1) || ((q->coded >> bq) & 1)) return 2;
-	int p0 = p->ref_idx[0][bp >> 2] < 0 ? -1 : p->ref_pic[0][bp >> 2], p1 = p->ref_idx[1][bp >> 2] < 0 ? -1 : p->ref_pic[1][bp >> 2];
-	int q0 = q->ref_idx[0][bq >> 2] < 0 ? -1 : q->ref_pic[0][bq >> 2], q1 = q->ref_idx[1][bq >> 2] < 0 ? -1 : q->ref_pic[1][bq >> 2];
-	if (!((p0 == q0 && p1 == q1) || (p0 == q1 && p1 == q0))) return 1;
-#define FAR(lp, lq) (dbk_iabs(p->mv[lp][bp][0] - q->mv[lq][bq][0]) >= 4 || dbk_iabs(p->mv[lp][bp][1] - q->mv[lq][bq][1]) >= 4)
-	if (p0 >= 0 && p1 >= 0) {
-		if (p0 != p1) return (p0 == q0) ? (FAR(0, 0) || FAR(1, 1)) : (FAR(0, 1) || FAR(1, 0));
-		return (FAR(0, 0) || FAR(1, 1)) && (FAR(0, 1) || FAR(1, 0));
-	}
-	int lp = p0 >= 0 ? 0 : 1, lq = q0 >= 0 ? 0 : 1;
-	return FAR(lp, lq);
-#undef FAR
+/* 8.7.2.1 for one edge segment between 4x4 blocks bp of p and bq of q.  Every candidate outcome is computed and the result
+ * is selected, so the 32 lanes of a digest (different edges, different cases) run one instruction stream; the records
+ * are read whole even where they do not matter (intra macroblocks), which is harmless. */
+__device__ __forceinline__ bool dbk_far(uint32_t a, uint32_t b) {      /* two packed quarter-sample vectors differ by 4 or more */
+	return dbk_iabs((int)(short)(a & 0xffffu) - (int)(short)(b & 0xffffu)) >= 4 || dbk_iabs((int)(short)(a >> 16) - (int)(short)(b >> 16)) >= 4;
+}
+__device__ __forceinline__ int dbk_bs_pair(const E264MbRec *p, int bp, const E264MbRec *q, int bq, bool mb_edge) {
+	const bool intra = p->kind != MBK_INTER || q->kind != MBK_INTER;
+	const bool coef = (((p->coded >> bp) | (q->coded >> bq)) & 1) != 0;
+	const int ip = bp >> 2, iq = bq >> 2;
+	const int p0 = p->ref_idx[0][ip] < 0 ? -1 : p->ref_pic[0][ip], p1 = p->ref_idx[1][ip] < 0 ? -1 : p->ref_pic[1][ip];
+	const int q0 = q->ref_idx[0][iq] < 0 ? -1 : q->ref_pic[0][iq], q1 = q->ref_idx[1][iq] < 0 ? -1 : q->ref_pic[1][iq];
+	const bool same = (p0 == q0 && p1 == q1) || (p0 == q1 && p1 == q0);
+	const uint32_t pm0 = *(const uint32_t *)p->mv[0][bp], pm1 = *(const uint32_t *)p->mv[1][bp];
+	const uint32_t qm0 = *(const uint32_t *)q->mv[0][bq], qm1 = *(const uint32_t *)q->mv[1][bq];
+	const bool f00 = dbk_far(pm0, qm0), f11 = dbk_far(pm1, qm1), f01 = dbk_far(pm0, qm1), f10 = dbk_far(pm1, qm0);
+	const bool straight = f00 || f11, crossed = f01 || f10;
+	/* both lists: distinct pictures pair the vectors by picture, the same picture twice needs both pairings to differ;
+	 * one list: the vectors of the lists in use */
+	const bool one = p0 >= 0 ? (q0 >= 0 ? f00 : f01) : (q0 >= 0 ? f10 : f11);
+	const bool mv = p0 >= 0 && p1 >= 0 ? (p0 != p1 ? (p0 == q0 ? straight : crossed) : straight && crossed) : one;
+	return intra ? (mb_edge ? 4 : 3) : coef ? 2 : !same ? 1 : (int)mv;
 }
 
 /* digest of one macroblock by one warp: 32 boundary strengths (one lane per edge segment), thresholds of the nine plane x
- * edge-kind combinations.  recs: 3 x 12 uint4 of shared memory for the warp, dg: 64 bytes of shared memory. */
-__device__ __forceinline__ void dbk_digest_mb(const PicJob &J, uint4 (*recs)[12], E264DbkMb *dg, int mb, int lane) {
-	const int W = J.w_mbs, mbx = mb % W, mby = mb / W;
-	const E264MbRec *q = (const E264MbRec *)recs[0], *pL = (const E264MbRec *)recs[1], *pT = (const E264MbRec *)recs[2];
-	if (lane < 12) recs[0][lane] = __ldg((const uint4 *)(J.recs + mb) + lane);
-	else if (lane < 24) { if (mbx > 0) recs[1][lane - 12] = __ldg((const uint4 *)(J.recs + mb - 1) + lane - 12); }
-	if (lane < 12 && mby > 0) recs[2][lane] = __ldg((const uint4 *)(J.recs + mb - W) + lane);
-	__syncwarp();
+ * edge-kind combinations.  q, pL, pT: records of the macroblock and of its left and top neighbours in shared memory (pL /
+ * pT are read only where the macroblock's flags say that edge is filtered, but must point at readable memory);
+ * dg: 64 bytes of shared memory. */
+__device__ __forceinline__ void dbk_digest_mb(const PicJob &J, const E264MbRec *q, const E264MbRec *pL, const E264MbRec *pT, E264DbkMb *dg, int mb, int lane) {
 	const int qflags = q->flags;
 	const bool on_mb = qflags & MBF_DEBLOCK, fl = qflags & MBF_EDGE_L, ft = qflags & MBF_EDGE_T, t8 = qflags & MBF_T8x8;
-	int bs = 0;
+	int bs;
 	{
 		const int dir = lane >> 4, e = (lane >> 2) & 3, k = lane & 3;
-		const E264MbRec *p = q;
-		bool on = on_mb && !(t8 && (e & 1));
-		if (e == 0) { on = on && (dir ? ft : fl); p = dir ? pT : pL; }
-		if (on) {
-			const int qx = dir ? k : e, qy = dir ? e : k;
-			const int px_ = dir ? k : (e ? e - 1 : 3), py_ = dir ? (e ? e - 1 : 3) : k;
-			bs = dbk_bs_pair(p, blk_z(px_, py_), q, blk_z(qx, qy), e == 0);
-		}
+		const bool on = on_mb && !(t8 && (e & 1)) && (e != 0 || (dir ? ft : fl));
+		const E264MbRec *p = e != 0 ? q : dir ? pT : pL;
+		const int qx = dir ? k : e, qy = dir ? e : k;
+		const int px_ = dir ? k : (e - 1) & 3, py_ = dir ? (e - 1) & 3 : k;
+		const int b = dbk_bs_pair(p, blk_z(px_, py_), q, blk_z(qx, qy), e == 0);
+		bs = on ? b : 0;
 	}
 	unsigned v = (unsigned)bs << ((lane & 7) * 4);
 	v |= __shfl_xor_sync(0xffffffffu, v, 1); v |= __shfl_xor_sync(0xffffffffu, v, 2); v |= __shfl_xor_sync(0xffffffffu, v, 4);
 	if ((lane & 7) == 0) dg->bs[lane >> 3] = v;
 	if (lane < 9) {
-		const int pl = lane / 3, kind = lane % 3;
-		const E264MbRec *p = kind == 0 ? q : kind == 1 ? pL : pT;
-		if ((kind == 1 && !fl) || (kind == 2 && !ft) || !on_mb) p = q;
+		const int pl = (lane * 11) >> 5, kind = lane - 3 * pl;      /* lane / 3, lane % 3 for lane < 9 */
+		const bool nb = on_mb && (kind == 1 ? fl : kind == 2 && ft);
+		const E264MbRec *p = !nb ? q : kind == 1 ? pL : pT;
 		const E264SliceRec *sr = J.slices + q->slice_idx;
 		const int qpav = (p->qp[pl] + q->qp[pl] + 1) >> 1;
 		const int ia = min(max(qpav + sr->filter_offset_a, 0), 51), ib = min(max(qpav + sr->filter_offset_b, 0), 51);

@@ -112,7 +112,8 @@ struct __align__(16) InterSmem {
 	uint16_t queue[6][INTER_CHUNK * 32];           /* item = macroblock << 5 | list << 4 | luma4x4BlkIdx */
 	int qn[6];
 	WarpSmem ws[INTER_WARPS];
-	uint4 drecs[INTER_WARPS][3][12];               /* deblocking digests: records of the current, left and top macroblock per warp */
+	uint4 trec4[INTER_CHUNK][12];                  /* deblocking digests: the records of the row above the chunk's macroblocks */
+	uint4 lrec4[12];                               /* and the record left of its first macroblock */
 	E264DbkMb ddg[INTER_WARPS];
 	int16_t coef[INTER_WARPS][2][RES_COEF_MAX];
 	unsigned long long bars[INTER_WARPS][2];
@@ -171,15 +172,23 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 	}
 	unsigned parity[2] = {0, 0};
+	PT_DECL
 	const int nchunks = (nmb + INTER_CHUNK - 1) / INTER_CHUNK;
 	for (int chunk = blockIdx.x; chunk < nchunks; chunk += gridDim.x) {
 		const int mb0 = chunk * INTER_CHUNK, cnt = min(INTER_CHUNK, nmb - mb0);
 		__syncthreads();                               /* the previous chunk's predictions and records are no longer read */
+		PT_MARK(2)      /* block barriers */
 		/* ---- 1. records, queues ---- */
 		for (int i = tid; i < cnt * 12; i += INTER_WARPS * 32) sm.rec4[i / 12][i % 12] = __ldg((const uint4 *)(J.recs + mb0) + i);
+		if (J.dbk != nullptr) {      /* the neighbour records the digests read, loaded with the chunk's own (the top edge row has none) */
+			for (int i = tid; i < cnt * 12; i += INTER_WARPS * 32) if (mb0 + i / 12 >= J.w_mbs) sm.trec4[i / 12][i % 12] = __ldg((const uint4 *)(J.recs + mb0 - J.w_mbs) + i);
+			if (tid < 12 && mb0 > 0) sm.lrec4[tid] = __ldg((const uint4 *)(J.recs + mb0 - 1) + tid);
+		}
 		if (tid < 6) sm.qn[tid] = 0;
+		PT_MARK(0)      /* records and queues */
 		__syncthreads();
-		/* the macroblocks this warp finishes in step 3 are w, w + 4, ...: get the first coefficient run under way */
+		PT_MARK(2)
+		/* the macroblocks this warp finishes in step 3 are w, w + INTER_WARPS, ...: get the first coefficient run under way */
 		auto coef_issue = [&](int m, int b) -> int {     /* 0 not inter, 1 inter, 2 inter with coefficients (copy in flight) */
 			if (m >= cnt) return 0;
 			const E264MbRec *r = (const E264MbRec *)sm.rec4[m];
@@ -206,7 +215,9 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 			base = __shfl_sync(0xffffffffu, base, leader);
 			if (cls >= 0) sm.queue[cls][base + __popc(peers & ((1u << lane) - 1))] = (uint16_t)item;
 		}
+		PT_MARK(0)
 		__syncthreads();
+		PT_MARK(2)
 		/* ---- 2. one class at a time, 32 items per warp pass: the groups of all classes form one list ---- */
 		{
 			int total = 0;
@@ -221,16 +232,20 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 				if (k < sm.qn[c]) inter_item(J, sm, c, sm.queue[c][k], mb0, W, H);
 			}
 		}
+		PT_MARK(1)      /* prediction passes */
 		__syncthreads();
+		PT_MARK(2)
 		/* ---- 3. a warp per macroblock: inverse transform, weighting, residual, store ---- */
 		int b = 0;
 		bool failed = false;
 #pragma unroll 1
 		for (int m = w; m < cnt; m += INTER_WARPS, b ^= 1) {
 			const int what2 = coef_issue(m + INTER_WARPS, b ^ 1);
-			/* the macroblock's deblocking digest (every macroblock, intra ones too): record-only work whose loads of the
-			 * neighbour records are in flight together with the coefficient run requested above */
-			if (J.dbk != nullptr) dbk_digest_mb(J, sm.drecs[w], &sm.ddg[w], mb0 + m, lane);
+			/* the macroblock's deblocking digest (every macroblock, intra ones too), from the records in shared memory, while
+			 * the coefficient run requested above is in flight */
+			if (J.dbk != nullptr)
+				dbk_digest_mb(J, (const E264MbRec *)sm.rec4[m], (const E264MbRec *)(m > 0 ? sm.rec4[m - 1] : sm.lrec4), (const E264MbRec *)sm.trec4[m], &sm.ddg[w], mb0 + m, lane);
+			PT_MARK(3)          /* deblocking digest */
 			if (what) {
 				const int mb = mb0 + m, mbx = mb % J.w_mbs, mby = mb / J.w_mbs;
 				const E264MbRec *r = (const E264MbRec *)sm.rec4[m];
@@ -238,54 +253,46 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 				if (what == 2) {
 					if (!mbar_wait(&sm.bars[w][b], parity[b])) { if (lane == 0) atomicExch(J.err, 4u); failed = true; }
 					parity[b] ^= 1;
+					PT_MARK(4)  /* waiting for the coefficient run */
 					if (!failed) residual_stage(ws, r, sr, sm.coef[w][b], lane);
+					PT_MARK(5)  /* dequantisation and inverse transforms */
 				}
-				if (lane < 16 && !failed) {
-					const int z = lane, bx = blk_x(z), by = blk_y(z), i8 = z >> 2;
+				if (!failed) {
+					/* two lanes per 4x4 block: lane z + 16 h takes luma rows 2 h and 2 h + 1 of block z and its 2x2 samples of
+					 * chroma plane h (Cb, Cr) */
+					const int z = lane & 15, h = lane >> 4, bx = blk_x(z), by = blk_y(z), i8 = z >> 2;
 					const int r0 = r->ref_idx[0][i8], r1 = r->ref_idx[1][i8];
-					uint32_t py[4] = {0, 0, 0, 0}, pcb = 0, pcr = 0, qy[4] = {0, 0, 0, 0}, qcb = 0, qcr = 0;
-					if (r0 >= 0) { const uint4 a = *(const uint4 *)sm.pred[m][0][z]; const uint2 c2 = *(const uint2 *)(sm.pred[m][0][z] + 4); py[0] = a.x; py[1] = a.y; py[2] = a.z; py[3] = a.w; pcb = c2.x; pcr = c2.y; }
-					if (r1 >= 0) { const uint4 a = *(const uint4 *)sm.pred[m][1][z]; const uint2 c2 = *(const uint2 *)(sm.pred[m][1][z] + 4); qy[0] = a.x; qy[1] = a.y; qy[2] = a.z; qy[3] = a.w; qcb = c2.x; qcr = c2.y; }
+					uint32_t py[2] = {0, 0}, pc = 0, qy[2] = {0, 0}, qc = 0;
+					if (r0 >= 0) { const uint2 a = *(const uint2 *)(sm.pred[m][0][z] + 2 * h); py[0] = a.x; py[1] = a.y; pc = sm.pred[m][0][z][4 + h]; }
+					if (r1 >= 0) { const uint2 a = *(const uint2 *)(sm.pred[m][1][z] + 2 * h); qy[0] = a.x; qy[1] = a.y; qc = sm.pred[m][1][z][4 + h]; }
 					const int wpm = sr->wp_mode;
 					const bool bi = r0 >= 0 && r1 >= 0;
-					if (!bi && r0 < 0) {
-#pragma unroll
-						for (int k = 0; k < 4; k++) py[k] = qy[k];
-						pcb = qcb; pcr = qcr;
-					}
+					if (!bi && r0 < 0) { py[0] = qy[0]; py[1] = qy[1]; pc = qc; }
 					if (bi && wpm == WP_DEFAULT) {
-#pragma unroll
-						for (int k = 0; k < 4; k++) py[k] = mc_avg4(py[k], qy[k]);
-						pcb = mc_avg4(pcb, qcb); pcr = mc_avg4(pcr, qcr);
+						py[0] = mc_avg4(py[0], qy[0]); py[1] = mc_avg4(py[1], qy[1]); pc = mc_avg4(pc, qc);
 					} else if ((bi && wpm != WP_DEFAULT) || (wpm == WP_EXPLICIT && (r0 >= 0 || r1 >= 0))) {
-						/* one weighting body for every scheme: parameters per plane, then six words */
-						int wa[3], wb[3], o[3], sh[3], rnd[3];
+						/* one weighting body for every scheme: parameters of luma and of this lane's chroma plane, then three words */
+						int wa[2], wb[2], o[2], sh[2], rnd[2];
 						const int ll = r0 >= 0 ? 0 : 1, ri = (ll ? r1 : r0) & 15;
 #pragma unroll
-						for (int c = 0; c < 3; c++) {
-							const int lw = c ? sr->chroma_log2_wd : sr->luma_log2_wd;
-							if (bi && wpm == WP_EXPLICIT) { wa[c] = sr->wp_w[0][r0 & 15][c]; wb[c] = sr->wp_w[1][r1 & 15][c]; o[c] = (sr->wp_o[0][r0 & 15][c] + sr->wp_o[1][r1 & 15][c] + 1) >> 1; sh[c] = lw + 1; rnd[c] = 1 << lw; }
-							else if (bi) { wb[c] = sr->implicit_w1[r0 & 15][r1 & 15]; wa[c] = 64 - wb[c]; o[c] = 0; sh[c] = 6; rnd[c] = 32; }
-							else { wa[c] = sr->wp_w[ll][ri][c]; wb[c] = 0; o[c] = sr->wp_o[ll][ri][c]; sh[c] = lw; rnd[c] = lw >= 1 ? 1 << (lw - 1) : 0; }
+						for (int k = 0; k < 2; k++) {
+							const int c = k ? 1 + h : 0, lw = k ? sr->chroma_log2_wd : sr->luma_log2_wd;
+							if (bi && wpm == WP_EXPLICIT) { wa[k] = sr->wp_w[0][r0 & 15][c]; wb[k] = sr->wp_w[1][r1 & 15][c]; o[k] = (sr->wp_o[0][r0 & 15][c] + sr->wp_o[1][r1 & 15][c] + 1) >> 1; sh[k] = lw + 1; rnd[k] = 1 << lw; }
+							else if (bi) { wb[k] = sr->implicit_w1[r0 & 15][r1 & 15]; wa[k] = 64 - wb[k]; o[k] = 0; sh[k] = 6; rnd[k] = 32; }
+							else { wa[k] = sr->wp_w[ll][ri][c]; wb[k] = 0; o[k] = sr->wp_o[ll][ri][c]; sh[k] = lw; rnd[k] = lw >= 1 ? 1 << (lw - 1) : 0; }
 						}
-#pragma unroll
-						for (int k = 0; k < 4; k++) py[k] = wp_word(py[k], qy[k], wa[0], wb[0], rnd[0], sh[0], o[0]);
-						pcb = wp_word(pcb, qcb, wa[1], wb[1], rnd[1], sh[1], o[1]); pcr = wp_word(pcr, qcr, wa[2], wb[2], rnd[2], sh[2], o[2]);
+						py[0] = wp_word(py[0], qy[0], wa[0], wb[0], rnd[0], sh[0], o[0]); py[1] = wp_word(py[1], qy[1], wa[0], wb[0], rnd[0], sh[0], o[0]);
+						pc = wp_word(pc, qc, wa[1], wb[1], rnd[1], sh[1], o[1]);
 					}
 					if (what == 2) {
-#pragma unroll
-						for (int k = 0; k < 4; k++) py[k] = add_res4(py[k], ws->res + (by * 4 + k) * 16 + bx * 4);
-						const int16_t *rc = ws->res + 256 + (by * 2) * 8 + bx * 2;
-						const uint32_t a = *(const uint32_t *)rc, bb = *(const uint32_t *)(rc + 8), c2 = *(const uint32_t *)(rc + 64), d = *(const uint32_t *)(rc + 72);
-						pcb = mc_pack4(clip255((short)((int)(pcb & 255) + (short)(a & 0xffff))), clip255((short)((int)((pcb >> 8) & 255) + (short)(a >> 16))),
-						               clip255((short)((int)((pcb >> 16) & 255) + (short)(bb & 0xffff))), clip255((short)((int)(pcb >> 24) + (short)(bb >> 16))));
-						pcr = mc_pack4(clip255((short)((int)(pcr & 255) + (short)(c2 & 0xffff))), clip255((short)((int)((pcr >> 8) & 255) + (short)(c2 >> 16))),
-						               clip255((short)((int)((pcr >> 16) & 255) + (short)(d & 0xffff))), clip255((short)((int)(pcr >> 24) + (short)(d >> 16))));
+						const int16_t *ry = ws->res + (by * 4 + 2 * h) * 16 + bx * 4, *rc = ws->res + 256 + h * 64 + (by * 2) * 8 + bx * 2;
+						py[0] = add_res4(py[0], ry); py[1] = add_res4(py[1], ry + 16);
+						const uint32_t a = *(const uint32_t *)rc, bb = *(const uint32_t *)(rc + 8);
+						pc = mc_pack4(clip255((short)((int)(pc & 255) + (short)(a & 0xffff))), clip255((short)((int)((pc >> 8) & 255) + (short)(a >> 16))),
+						              clip255((short)((int)((pc >> 16) & 255) + (short)(bb & 0xffff))), clip255((short)((int)(pc >> 24) + (short)(bb >> 16))));
 					}
-#pragma unroll
-					for (int k = 0; k < 4; k++) *(uint32_t *)&YT(bx * 4, by * 4 + k) = py[k];
-					*(uint16_t *)&CT(0, bx * 2, by * 2) = (uint16_t)pcb; *(uint16_t *)&CT(0, bx * 2, by * 2 + 1) = (uint16_t)(pcb >> 16);
-					*(uint16_t *)&CT(1, bx * 2, by * 2) = (uint16_t)pcr; *(uint16_t *)&CT(1, bx * 2, by * 2 + 1) = (uint16_t)(pcr >> 16);
+					*(uint32_t *)&YT(bx * 4, by * 4 + 2 * h) = py[0]; *(uint32_t *)&YT(bx * 4, by * 4 + 2 * h + 1) = py[1];
+					*(uint16_t *)&CT(h, bx * 2, by * 2) = (uint16_t)pc; *(uint16_t *)&CT(h, bx * 2, by * 2 + 1) = (uint16_t)(pc >> 16);
 				}
 				__syncwarp();
 				if (!failed) {
@@ -294,7 +301,9 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 				}
 				__syncwarp();
 			}
+			PT_MARK(6)      /* combination, residual, stores */
 			what = what2;
 		}
 	}
+	PT_FLUSH(16)
 }

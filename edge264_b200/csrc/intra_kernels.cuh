@@ -27,7 +27,7 @@ struct __align__(16) IntraRowsSmem {
 	uint32_t ring[IR_ROWS][IR_RING][8];         /* bottom sample row of a finished macroblock: luma (4 words), Cb (2), Cr (2) */
 	int16_t coef[IR_ROWS][IR_SLOTS][RES_COEF_MAX];   /* coefficient runs of macroblocks x .. x+3 of every row (cp.async.bulk) */
 	unsigned long long bars[IR_ROWS][IR_SLOTS];
-	uint4 drecs[IR_ROWS][3][12];                /* deblocking digests of intra-only pictures: current, left and top record */
+	uint4 drecs[IR_ROWS][12];                   /* deblocking digests of intra-only pictures: the top neighbour's record */
 	E264DbkMb ddg[IR_ROWS];
 	int done[IR_ROWS];                          /* macroblocks a row has put into its ring */
 	int taken[IR_ROWS];                         /* the macroblock a row is working on: ring entries before it (minus one) are free */
@@ -62,7 +62,9 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 		return true;
 	};
 	unsigned pending = 0;                        /* bit x % IR_SLOTS: macroblock x has a copy in flight */
-	RT_DECL
+	uint4 topreg = make_uint4(0, 0, 0, 0);       /* digests: the top neighbour's record, one macroblock ahead */
+	if (digests && mby > 0 && lane < 12) topreg = __ldg((const uint4 *)(rowrecs - W) + lane);
+	PT_DECL
 	for (int x = 0; x < AHEAD && x < W; x++) if (coef_issue(x)) pending |= 1u << (x % IR_SLOTS);
 #pragma unroll 1
 	for (int mbx = 0; mbx < W; mbx++) {
@@ -76,7 +78,7 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 			__threadfence_block();
 		}
 		__syncwarp();
-		RT_MARK(0)      /* waiting for a free slot */
+		PT_MARK(0)      /* waiting for a free slot */
 		const E264MbRec *r = (const E264MbRec *)sm.recs[w][mbx % IR_RECS];
 		WarpSmem *ws = &sm.ws[w][sl];
 		/* the record fetched one iteration ago goes to shared memory, the next one is requested */
@@ -85,11 +87,11 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 		__syncwarp();
 		if (mbx + AHEAD < W) { const int nb = (mbx + AHEAD) % IR_SLOTS; pending &= ~(1u << nb); if (coef_issue(mbx + AHEAD)) pending |= 1u << nb; }
 		const int kind = r->kind;
-		RT_MARK(1)      /* records, coefficient copy issued */
+		PT_MARK(1)      /* records, coefficient copy issued */
 		if ((pending >> sl) & 1) {
 			if (!mbar_wait(&sm.bars[w][sl], (parbits >> sl) & 1)) { if (lane == 0) atomicExch(J.err, 3u); }
 			parbits ^= 1u << sl;
-			RT_MARK(2)  /* waiting for the coefficient run */
+			PT_MARK(2)  /* waiting for the coefficient run */
 			residual_stage(ws, r, J.slices + r->slice_idx, sm.coef[w][sl], lane);
 		} else if (kind != MBK_INTER && kind != MBK_IPCM) {
 			((uint4 *)ws->res)[lane] = make_uint4(0, 0, 0, 0);
@@ -97,11 +99,16 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 		}
 		__syncwarp();
 		if (lane == 0) { __threadfence_block(); *ready = mbx + 1; }
-		RT_MARK(3)      /* inverse transforms */
-		if (digests) dbk_digest_mb(J, sm.drecs[w], &sm.ddg[w], mby * W + mbx, lane);
-		RT_MARK(4)      /* deblocking digest */
+		PT_MARK(3)      /* inverse transforms */
+		if (digests) {      /* the macroblock's record and the left one are in the record ring */
+			if (lane < 12) sm.drecs[w][lane] = topreg;
+			if (mby > 0 && mbx + 1 < W && lane < 12) topreg = __ldg((const uint4 *)(rowrecs - W + mbx + 1) + lane);
+			__syncwarp();
+			dbk_digest_mb(J, r, (const E264MbRec *)sm.recs[w][(mbx + IR_RECS - 1) % IR_RECS], (const E264MbRec *)sm.drecs[w], &sm.ddg[w], mby * W + mbx, lane);
+		}
+		PT_MARK(4)      /* deblocking digest */
 	}
-	RT_FLUSH(0)
+	PT_FLUSH(0)
 }
 
 /* The row's PREDICTION warp: waits for the residual, for the row above (top-right neighbour finished) and for room in
@@ -125,7 +132,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 	uint8_t *dst = J.frames + (size_t)J.dst_slot * J.frame_bytes;
 	const int cpl = J.stride_c >> 1;
 	int avail = 0;                                            /* macroblocks of the row above the band known to be stored */
-	RT_DECL
+	PT_DECL
 #pragma unroll 1
 	for (int mbx = 0; mbx < W; mbx++) {
 		uint8_t *Y = dst + (size_t)(mby * 16) * J.stride_y + mbx * 16;
@@ -134,7 +141,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 		if (lane == 0) {
 			unsigned spins = 0; bool bad = false;
 			while (*ready <= mbx && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
-			RT_MARK(0)  /* waiting for the residual */
+			PT_MARK(0)  /* waiting for the residual */
 			const int need = min(mbx + 2, W);
 			if (from_ring) {
 				while (*done_in < need && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
@@ -145,7 +152,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 				__threadfence();
 				avail = bad ? W : (int)(v - base);
 			}
-			RT_MARK(1)  /* waiting for the row above */
+			PT_MARK(1)  /* waiting for the row above */
 			if (to_ring) while (*taken_next <= mbx - IR_RING + 1 && !bad)     /* entry mbx - RING is still the corner sample of the row below's macroblock mbx - RING + 1 */ { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
 			if (bad) atomicExch(J.err, 1u);
 			__threadfence_block();
@@ -169,7 +176,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 			if (lane < 18) { const int pl = lane / 9, cx = lane % 9 - 1; if (cx >= 0 || mbx > 0) CT(pl, cx, -1) = __ldcg(C + pl * cpl - J.stride_c + cx); }
 		}
 		__syncwarp();
-		RT_MARK(2)      /* ring room, hand-shake, row above into the tile */
+		PT_MARK(2)      /* ring room, hand-shake, row above into the tile */
 		/* ---- the macroblock ---- */
 		if (kind == MBK_INTER) {   /* reconstructed by the inter kernel: fetch its right column and bottom row for the neighbours to come */
 			if (lane < 16) YT(15, lane) = __ldcg(Y + (size_t)lane * J.stride_y + 15);
@@ -186,9 +193,9 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 				__syncwarp();
 			} else {
 				intra_luma(ws, r, lane);
-				RT_MARK(3)  /* luma prediction */
+				PT_MARK(3)  /* luma prediction */
 				intra_chroma(ws, r, lane);
-				RT_MARK(4)  /* chroma prediction */
+				PT_MARK(4)  /* chroma prediction */
 			}
 			store_mb(ws, J, Y, C, lane);
 			if (to_ring) {
@@ -197,7 +204,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 			}
 		}
 		__syncwarp();
-		RT_MARK(5)      /* stores */
+		PT_MARK(5)      /* stores */
 		/* ---- publish: shared-memory counter for the row below in this band; global counter for the next band, one chunk late ---- */
 		if (lane == 0) {
 			if (to_ring) { __threadfence_block(); *done_out = mbx + 1; }
@@ -213,9 +220,9 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 		__syncwarp();
 		if (lane == 0) { __threadfence_block(); *used = mbx + 1; }
 		avail = __shfl_sync(0xffffffffu, avail, 0);
-		RT_MARK(6)      /* publication, column hand-over */
+		PT_MARK(6)      /* publication, column hand-over */
 	}
-	RT_FLUSH(8)
+	PT_FLUSH(8)
 	__syncwarp();
 	if (lane == 0) {
 		*taken_me = W + IR_RING;       /* nothing of the ring above is needed any more */

@@ -432,7 +432,7 @@ extern "C" int e264b_replay(E264bDevice **cs, int n, int reps, int threads, E264
 	 * for the driver) would otherwise bound the result.  The synchronisation words restart at every repetition
 	 * (two memset nodes) because the captured epochs repeat.  E264B_REPLAY_GRAPH=0 issues plain launches instead. */
 	const int diag = getenv("E264B_DIAG") && atoi(getenv("E264B_DIAG")) ? 1 : 0;
-	if (diag) { static unsigned long long zp[16]; cudaMemcpyToSymbol(g_diag_phase, zp, sizeof zp); }
+	if (diag) { static unsigned long long zp[24]; cudaMemcpyToSymbol(g_diag_phase, zp, sizeof zp); }
 	if (diag) { static unsigned z[3][4][160]; cudaMemcpyToSymbol(g_diag_cnt, z[0], sizeof z[0]); cudaMemcpyToSymbol(g_diag_cur, z[1], sizeof z[1]); cudaMemcpyToSymbol(g_diag_max, z[2], sizeof z[2]); }
 	const char *ge = getenv("E264B_REPLAY_GRAPH");
 	const bool use_graph = !(ge && atoi(ge) == 0);
@@ -526,14 +526,18 @@ extern "C" int e264b_replay(E264bDevice **cs, int n, int reps, int threads, E264
 			fprintf(stderr, "\n");
 		}
 	}
-	if (diag) {     /* -DE264_ROWS_TIMING builds: cycles per part of a macroblock step in the intra-picture kernel, all warps summed */
-		unsigned long long ph[16]; cudaMemcpyFromSymbol(ph, g_diag_phase, sizeof ph);
-		unsigned long long tt = 0, tp = 0; for (int k = 0; k < 8; k++) { tt += ph[k]; tp += ph[8 + k]; }
+	if (diag) {     /* -DE264_PHASE_TIMING builds: cycles per part of the work of the intra-picture and inter kernels, all warps summed */
+		unsigned long long ph[24]; cudaMemcpyFromSymbol(ph, g_diag_phase, sizeof ph);
+		unsigned long long tt = 0, tp = 0, ti = 0; for (int k = 0; k < 8; k++) { tt += ph[k]; tp += ph[8 + k]; ti += ph[16 + k]; }
 		if (tt + tp) {
 			const char *tn[8] = {"wait slot", "records+issue", "wait coefficients", "transforms", "digest", "-", "-", "-"};
 			const char *pn[8] = {"wait residual", "wait row above", "ring+hand-shake+tile", "luma", "chroma", "stores", "publish+column", "-"};
 			fprintf(stderr, "rows kernel, transform warps:"); for (int k = 0; k < 5; k++) fprintf(stderr, " %s %.1f%%", tn[k], 100.0 * ph[k] / (double)tt); fprintf(stderr, "\n");
 			fprintf(stderr, "rows kernel, prediction warps:"); for (int k = 0; k < 7; k++) fprintf(stderr, " %s %.1f%%", pn[k], 100.0 * ph[8 + k] / (double)tp); fprintf(stderr, "\n");
+		}
+		if (ti) {
+			const char *in_[8] = {"records+queues", "prediction passes", "block barriers", "digest", "wait coefficients", "residual", "combine+store", "-"};
+			fprintf(stderr, "inter kernel (%.3g G warp-cycles):", 1e-9 * (double)ti); for (int k = 0; k < 7; k++) fprintf(stderr, " %s %.1f%%", in_[k], 100.0 * ph[16 + k] / (double)ti); fprintf(stderr, "\n");
 		}
 	}
 	const char *trace_path = getenv("E264B_TRACE");

@@ -55,32 +55,22 @@ __device__ __forceinline__ int blk_x(int b) { return (b & 1) | ((b >> 1) & 2); }
 __device__ __forceinline__ int blk_y(int b) { return ((b >> 1) & 1) | ((b >> 2) & 2); }
 __device__ __forceinline__ int blk_z(int x, int y) { return (x & 1) | ((y & 1) << 1) | ((x & 2) << 1) | ((y & 2) << 2); }
 __device__ __forceinline__ int norm4(int m, int i, int j) { return h264_norm4x4[m][((i & 1) && (j & 1)) ? 1 : (!(i & 1) && !(j & 1)) ? 0 : 2]; }
-__device__ __forceinline__ int norm8(int m, int i, int j) {
-	int k;
-	if (!(i & 3) && !(j & 3)) k = 0;
-	else if ((i & 1) && (j & 1)) k = 1;
-	else if ((i & 3) == 2 && (j & 3) == 2) k = 2;
-	else if ((!(i & 3) && (j & 1)) || ((i & 1) && !(j & 3))) k = 3;
-	else if ((!(i & 3) && (j & 3) == 2) || ((i & 3) == 2 && !(j & 3))) k = 4;
-	else k = 5;
-	return h264_norm8x8[m][k];
-}
-
 __device__ __forceinline__ void reset_next_tickets(const PicJob &J) { if (blockIdx.x == 0 && threadIdx.x < 4) J.tickets_next[threadIdx.x] = 0; }
 
 /* measurement only (replay with E264B_DIAG=1): how the blocks of each kernel kind land on the SMs —
  * [kind][sm]: blocks started, blocks of this kind resident right now, the maximum of that */
 __device__ unsigned g_diag_cnt[4][160], g_diag_cur[4][160], g_diag_max[4][160];
-/* -DE264_ROWS_TIMING (make variants): SM cycles the warps of e264_intra_rows_kernel spend per part of a macroblock step */
-__device__ unsigned long long g_diag_phase[16];
-#ifdef E264_ROWS_TIMING
-#define RT_DECL unsigned rt_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}; unsigned rt_t = (unsigned)clock64();
-#define RT_MARK(k) { const unsigned rt_n = (unsigned)clock64(); rt_acc[k] += rt_n - rt_t; rt_t = rt_n; }
-#define RT_FLUSH(base) if (lane == 0) { for (int rt_k = 0; rt_k < 8; rt_k++) atomicAdd(&g_diag_phase[(base) + rt_k], (unsigned long long)rt_acc[rt_k]); }
+/* -DE264_PHASE_TIMING (make variants): SM cycles the warps of a kernel spend per part of its work, all warps summed —
+ * [0..7] transform warps and [8..15] prediction warps of e264_intra_rows_kernel, [16..23] warps of e264_inter4_kernel */
+__device__ unsigned long long g_diag_phase[24];
+#ifdef E264_PHASE_TIMING
+#define PT_DECL unsigned pt_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}; unsigned pt_t = (unsigned)clock64();
+#define PT_MARK(k) { const unsigned pt_n = (unsigned)clock64(); pt_acc[k] += pt_n - pt_t; pt_t = pt_n; }
+#define PT_FLUSH(base) if (lane == 0) { for (int pt_k = 0; pt_k < 8; pt_k++) atomicAdd(&g_diag_phase[(base) + pt_k], (unsigned long long)pt_acc[pt_k]); }
 #else
-#define RT_DECL
-#define RT_MARK(k)
-#define RT_FLUSH(base)
+#define PT_DECL
+#define PT_MARK(k)
+#define PT_FLUSH(base)
 #endif
 /* measurement only: first-start / last-end timestamps of a launch, see e264b_replay */
 struct TraceScope {
@@ -141,7 +131,8 @@ __device__ __forceinline__ bool mbar_wait(void *bar, unsigned parity) {
 /* residual                                                                                     */
 /* ------------------------------------------------------------------------------------------ */
 /* 4x4 inverse transform of 16 levels at c (16-byte aligned) -> residual written to dst[y*dstride+x] */
-static_assert(offsetof(E264SliceRec, scaling4x4) % 8 == 0 && sizeof(E264SliceRec) % 8 == 0, "idct4x4 loads a 4x4 scaling list as two 8-byte words");
+static_assert(offsetof(E264SliceRec, scaling4x4) % 8 == 0 && offsetof(E264SliceRec, scaling8x8) % 8 == 0 && sizeof(E264SliceRec) % 8 == 0,
+              "idct4x4 loads a 4x4 scaling list as two 8-byte words, residual_stage a row of an 8x8 list as one");
 __device__ __noinline__ void idct4x4(const int16_t *c, bool have_levels, const uint8_t *scaling, int qp, bool dc_override, int dc, int16_t *dst, int dstride) {
 	int d[16];
 	if (have_levels) {
@@ -251,10 +242,15 @@ __device__ __noinline__ void residual_stage(WarpSmem *ws, const E264MbRec *r, co
 			uint4 q = *(const uint4 *)(cf_luma + idx * 64 + k * 8);
 			short lv[8]; *(uint4 *)lv = q;
 			int div = qpy / 6, m = qpy - div * 6;
-			const uint8_t *sc = sr->scaling8x8[inter] + k * 8;
+			/* normAdjust8x8 of row k takes three values: one for columns 0 and 4, one for the odd columns, one for
+			 * columns 2 and 6 (rows 0 and 4: classes 0 3 4, odd rows: 3 1 5, rows 2 and 6: 4 5 2) */
+			const uint8_t *nm = h264_norm8x8[m];
+			const int n0 = nm[0], n1 = nm[1], n2 = nm[2], n3 = nm[3], n4 = nm[4], n5 = nm[5];
+			const int v0 = (k & 1) ? n3 : (k & 2) ? n4 : n0, v1 = (k & 1) ? n1 : (k & 2) ? n5 : n3, v2 = (k & 1) ? n5 : (k & 2) ? n2 : n4;
+			const uint2 sw = __ldg((const uint2 *)(sr->scaling8x8[inter] + k * 8));
 #pragma unroll
 			for (int j = 0; j < 8; j++) {
-				int ls = sc[j] * norm8(m, k, j);
+				int ls = (int)(((j < 4 ? sw.x : sw.y) >> (8 * (j & 3))) & 255u) * ((j & 1) ? v1 : (j & 2) ? v2 : v0);
 				a[j] = div < 6 ? (short)sat16((lv[j] * ls + (1 << (5 - div))) >> (6 - div)) : (short)(lv[j] * (short)(ls << (div - 6)));
 			}
 			idct8_1d(a);
