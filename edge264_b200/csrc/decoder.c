@@ -987,10 +987,20 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 	if (h->slice_type < 2) {
 		int lists[2][32], nl[2];
 		build_ref_lists(d, h, lists, nl);
-		for (int l = 0; l <= (h->slice_type == 1); l++) for (int i = 0; i < h->num_ref[l]; i++) {
-			int sl = lists[l][i];
-			if (sl < 0) continue;   /* missing reference: MC will read slot -1 -> treated as the current slot by the backend */
-			c->ref_slot[l][i] = (int8_t)sl; c->ref_uid[l][i] = d->pics[sl].uid; c->ref_poc[l][i] = d->pics[sl].poc; c->ref_long[l][i] = d->pics[sl].ref == 2;
+		for (int l = 0; l <= (h->slice_type == 1); l++) {
+			/* a missing entry (damaged or non-conforming stream) is predicted from a defined picture other than the one
+			 * being decoded: the list's first present entry, else the picture concealment copies from.  It keeps
+			 * ref_uid -1, so direct prediction and implicit weights still see it as missing. */
+			int subst = -1;
+			for (int i = 0; i < h->num_ref[l] && subst < 0; i++) subst = lists[l][i];
+			if (subst < 0) subst = conceal_reference(d);
+			if (subst < 0) return EBADMSG;   /* nothing to predict from: the slice is not decoded */
+			for (int i = 0; i < h->num_ref[l]; i++) {
+				int sl = lists[l][i];
+				c->ref_slot[l][i] = (int8_t)(sl < 0 ? subst : sl);
+				if (sl < 0) continue;
+				c->ref_uid[l][i] = d->pics[sl].uid; c->ref_poc[l][i] = d->pics[sl].poc; c->ref_long[l][i] = d->pics[sl].ref == 2;
+			}
 		}
 		if (h->slice_type == 1 && lists[1][0] >= 0) {
 			c->col_recs = d->pics[lists[1][0]].recs;
@@ -1006,7 +1016,7 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 		if (wp == 2) {   /* 8.4.2.3.1 implicit weights from POC distances */
 			for (int i0 = 0; i0 < h->num_ref[0] && i0 < 16; i0++) for (int i1 = 0; i1 < h->num_ref[1] && i1 < 16; i1++) {
 				int w1 = 32;
-				if (c->ref_slot[0][i0] >= 0 && c->ref_slot[1][i1] >= 0 && !c->ref_long[0][i0] && !c->ref_long[1][i1]) {
+				if (c->ref_uid[0][i0] >= 0 && c->ref_uid[1][i1] >= 0 &&!c->ref_long[0][i0] && !c->ref_long[1][i1]) {
 					int poc0 = c->ref_poc[0][i0], poc1 = c->ref_poc[1][i1];
 					int tb = cp->poc_dec - poc0, td = poc1 - poc0;
 					tb = tb < -128 ? -128 : tb > 127 ? 127 : tb; td = td < -128 ? -128 : td > 127 ? 127 : td;

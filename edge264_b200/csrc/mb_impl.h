@@ -350,9 +350,10 @@ static void sx_macroblock(SliceCtx *s) {
 					int pred = sx_pred_intra_mode(s, (i8 & 1) * 2, (i8 >> 1) * 2);
 					int want = ENCV(SYN(ipm[i8 * 4]));
 					int rem = se_intra_pred_mode(s, ENCV(want == pred ? -1 : want < pred ? want : want - 1));
-					int mode = rem < 0 ? pred : rem + (rem >= pred);
+					int mode = rem < 0 ? pred : rem + (rem >= pred), un = sx_unavail8x8(s, i8);
+					if (!e264_intra_mode_legal(MBK_I8x8, mode, un)) { s->error = 1; mode = 2; }   /* reads a neighbour that is not there: DC */
 					memset(m->ipm + i8 * 4, mode, 4);
-					r->modes[i8] = IMODE(mode, sx_unavail8x8(s, i8));
+					r->modes[i8] = IMODE(mode, un);
 				}
 			} else {
 				r->kind = MBK_I4x4;
@@ -360,17 +361,21 @@ static void sx_macroblock(SliceCtx *s) {
 					int pred = sx_pred_intra_mode(s, e264_blk_x(b), e264_blk_y(b));
 					int want = ENCV(SYN(ipm[b]));
 					int rem = se_intra_pred_mode(s, ENCV(want == pred ? -1 : want < pred ? want : want - 1));
-					int mode = rem < 0 ? pred : rem + (rem >= pred);
+					int mode = rem < 0 ? pred : rem + (rem >= pred), un = sx_unavail4x4(s, b);
+					if (!e264_intra_mode_legal(MBK_I4x4, mode, un)) { s->error = 1; mode = 2; }
 					m->ipm[b] = (int8_t)mode;
-					r->modes[b] = IMODE(mode, sx_unavail4x4(s, b));
+					r->modes[b] = IMODE(mode, un);
 				}
 			}
 		} else {
 			m->is_i16 = 1; r->kind = MBK_I16x16;
-			r->i16_mode = IMODE((ityp - 1) & 3, sx_unavail16(s));
+			int mode = (ityp - 1) & 3;
+			if (!e264_intra_mode_legal(MBK_I16x16, mode, sx_unavail16(s))) { s->error = 1; mode = 2; }
+			r->i16_mode = IMODE(mode, sx_unavail16(s));
 		}
 		int cm = se_intra_chroma_pred_mode(s, ENCV(SYN(chroma_mode)));
 		if (cm > 3) { s->error = 1; return; }
+		if (!e264_intra_mode_legal(-1, cm, sx_unavail16(s))) { s->error = 1; cm = 0; }
 		m->chroma_pred_mode = (uint8_t)cm;
 		r->chroma_mode = IMODE(cm, sx_unavail16(s));
 		if (ityp == 0) cbp = se_coded_block_pattern(s, ENCV(SYN(cbp)), 1);

@@ -19,6 +19,29 @@
  *           or for each coded 8x8 block: 64 levels                 (transform 8x8; its 4 bits are set together)
  *           [4 Cb DC + 4 Cr DC levels, raster 2x2]                 if coded bit 25 or 26
  *           for each coded chroma AC block (Cb0..3 then Cr0..3): 16 levels (slot 0 unused, zero)
+ *
+ * The record contract: what the parser guarantees for every picture it submits, damaged input included, and what the
+ * kernels rely on (a record outside it may make a kernel read samples nobody wrote, or copy outside the coefficient
+ * pool).  oracle/record_check.c checks exactly this list (E264_CHECK_RECORDS=1 on the CPU restatement backend).
+ *   Picture   dst_slot < n_slots; 1 <= n_slices <= 64; intra_list holds the addresses of the non-inter macroblocks in
+ *             raster order and n_intra counts them; any_deblock is set when a macroblock has MBF_DEBLOCK.
+ *   Slices    filter_offset_a/b even in -12..12; deblock_idc 0..2; slice_type 0..2; wp_mode 0..2; log2_wd 0..7;
+ *             weights -128..128, offsets -128..127, implicit_w1 -64..128; scaling entries 1..255.
+ *   Kind      kind 0..4, flags inside MBF_*, slice_idx < n_slices, coded inside CODED_*.  MBF_T8x8 is set on every
+ *             MBK_I8x8 and never on MBK_I4x4, MBK_I16x16 or MBK_IPCM; with MBF_T8x8 the luma bits come in groups of 4.
+ *             CODED_Y_DC appears only on MBK_I16x16; MBK_IPCM has no coded bits.
+ *   QPs       qp[0] 0..51 (0 for MBK_IPCM); qp[1], qp[2] are values of Table 8-15 (0..39).
+ *   Levels    coef_off is a multiple of 8 and the run (192 slots for MBK_IPCM) ends inside n_coefs.
+ *   Intra     a neighbour that a mode byte marks available (bit clear) lies inside the picture and in the same slice
+ *             (slice_idx); C is always unavailable for the 4x4 blocks z = 3, 7, 11, 13, 15 and the 8x8 block 3.
+ *             The parser sets the bits of 6.4.11.4 exactly; a record may mark more neighbours unavailable than that
+ *             (the concealment records mark all of them).  Every mode is legal for its bits (e264_intra_mode_legal).
+ *   Deblock   MBF_EDGE_L / MBF_EDGE_T only with MBF_DEBLOCK, never on the picture's left column / top row; MBF_DEBLOCK
+ *             only in slices with deblock_idc != 1.  With deblock_idc 0 both edges are set wherever a neighbour exists,
+ *             with deblock_idc 2 an edge is set only towards a macroblock of the same slice.
+ *   Inter     every 8x8 block of an MBK_INTER uses at least one list; a used list has ref_idx 0..15 and a ref_pic in
+ *             [0, n_slots) other than dst_slot; an unused list, and every list of an intra macroblock, has -1 in both.
+ *             Motion vectors may take any int16 value.
  */
 #ifndef E264B_RECORDS_H
 #define E264B_RECORDS_H
@@ -111,5 +134,22 @@ typedef struct E264Staging {
 static inline int e264_blk_x(int b) { return ((b & 1) | ((b >> 1) & 2)); }          /* z-order -> 4x4 column */
 static inline int e264_blk_y(int b) { return (((b >> 1) & 1) | ((b >> 2) & 2)); }   /* z-order -> 4x4 row    */
 static inline int e264_blk_z(int x, int y) { return (x & 1) | ((y & 1) << 1) | ((x & 2) << 1) | ((y & 2) << 2); }
+
+/* whether a prediction mode only reads neighbours its unavailability bits (A=1, B=2, D=8) allow (8.3.1.2, 8.3.2.2,
+ * 8.3.3, 8.3.4); C is substituted when unavailable.  kind: MBK_I4x4 / MBK_I8x8 (mode 0..8), MBK_I16x16 (0..3), or
+ * -1 for the chroma mode (0..3).  DC is legal for every availability. */
+static inline int e264_intra_mode_legal(int kind, int mode, int un) {
+	if (kind == MBK_I4x4 || kind == MBK_I8x8) {
+		switch (mode) {
+		case 0: case 3: case 7: return !(un & 2);
+		case 1: case 8: return !(un & 1);
+		case 2: return 1;
+		case 4: case 5: case 6: return !(un & 11);
+		default: return 0;
+		}
+	}
+	if (kind == MBK_I16x16) return mode == 0 ? !(un & 2) : mode == 1 ? !(un & 1) : mode == 2 ? 1 : mode == 3 ? !(un & 11) : 0;
+	return mode == 0 ? 1 : mode == 1 ? !(un & 1) : mode == 2 ? !(un & 2) : mode == 3 ? !(un & 11) : 0;
+}
 
 #endif

@@ -19,7 +19,9 @@ int e264_parse_slice_data(SliceCtx *s) {
 		if (s->mbi[s->mbaddr].slice_id) { s->error = 1; break; }            /* already delivered by another slice of this picture */
 		if (s->n_coefs + 408u > s->coef_cap) { s->error = 2; break; }        /* a macroblock takes at most 16+256+8+128 levels: the pool cannot overflow inside it */
 		int end = sx_one_mb(s);
-		if (s->error) break;
+		/* a macroblock that failed to parse may have a partial record: it counts as not delivered, so the picture's
+		 * concealment (decoder.c conceal_missing) gives it a complete one */
+		if (s->error) { s->cur->slice_id = 0; break; }
 		n++;
 		if (s->cabac && cabac_dec_overrun(&s->cd)) { s->error = 1; break; }
 		if (!s->cabac && s->br.overrun) { s->error = 1; break; }

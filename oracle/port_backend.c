@@ -7,6 +7,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include "../edge264_b200/csrc/dec.h"
+#include "record_check.h"
 
 void port_recon_picture(uint8_t *frames, const E264PicDesc *pd, const E264MbRec *recs, const int16_t *coefs, const E264SliceRec *slices);
 
@@ -80,6 +81,15 @@ static int port_submit(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint
 	}
 	pic_no++;
 	if (pd->staging < 0 || pd->staging >= c->n_stage) return -1;
+	/* E264_CHECK_RECORDS=1: every submitted picture must keep the record contract (records.h); stop at the first violation */
+	const char *chk = getenv("E264_CHECK_RECORDS");
+	if (chk && atoi(chk)) {
+		char why[256];
+		if (e264_check_records(pd, c->recs[pd->dst_slot], c->coefs[pd->staging], c->slices[pd->staging], c->intra_list[pd->staging], c->n_slots, why, sizeof(why))) {
+			fprintf(stderr, "E264_CHECK_RECORDS: picture %d (slot %d): %s\n", pic_no - 1, pd->dst_slot, why);
+			abort();
+		}
+	}
 	if (!getenv("E264_NULL_RECON")) port_recon_picture(c->frames, pd, c->recs[pd->dst_slot], c->coefs[pd->staging], c->slices[pd->staging]);
 	if (!getenv("E264_NULL_RECON")) memcpy(host_out, c->frames + (size_t)pd->dst_slot * pd->frame_bytes, (size_t)pd->frame_bytes);
 	/* E264_PORT_LATE=n (tests of the decoder's output logic): pictures get tickets and count as "still on the device" until
