@@ -107,7 +107,7 @@ __device__ __forceinline__ void dbk_line_luma(int &p3, int &p2, int &p1, int &p0
 	const int avg = (p0 + q0 + 1) >> 1;
 	int n_p1 = p1 + min(max((p2 + avg - (p1 << 1)) >> 1, -tcp), tcp);
 	int n_q1 = q1 + min(max((q2 + avg - (q1 << 1)) >> 1, -tcq), tcq);
-	int n_p0 = min(max(p0 + d, 0), 255), n_q0 = min(max(q0 - d, 0), 255);
+	int n_p0 = mc_clip255(p0 + d), n_q0 = mc_clip255(q0 - d);
 	if (STRONG && any4) {   /* bS 4 exists only on macroblock edges; `any4` is uniform over the warp */
 		const bool s4 = f && bs == 4;
 		const bool small = ad < ((alpha >> 2) + 2);
@@ -128,8 +128,8 @@ __device__ __forceinline__ void dbk_line_chroma(int p1, int &p0, int &q0, int q1
 	const int tc = f ? tc0 + 1 : 0;
 	const int d = min(max((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc), tc);
 	const bool s4 = f && bs == 4;
-	const int n_p0 = s4 ? (2 * p1 + p0 + q1 + 2) >> 2 : min(max(p0 + d, 0), 255);
-	const int n_q0 = s4 ? (2 * q1 + q0 + p1 + 2) >> 2 : min(max(q0 - d, 0), 255);
+	const int n_p0 = s4 ? (2 * p1 + p0 + q1 + 2) >> 2 : mc_clip255(p0 + d);
+	const int n_q0 = s4 ? (2 * q1 + q0 + p1 + 2) >> 2 : mc_clip255(q0 - d);
 	p0 = n_p0; q0 = n_q0;
 }
 
@@ -148,7 +148,6 @@ struct __align__(16) DbkSmem {
 };
 
 __device__ __forceinline__ int dbk_byte(uint32_t w, int k) { return (int)((w >> (8 * k)) & 0xffu); }
-__device__ __forceinline__ uint32_t dbk_pack(int a, int b, int c, int d) { return (uint32_t)a | (uint32_t)b << 8 | (uint32_t)c << 16 | (uint32_t)d << 24; }
 
 /* One warp = one pair of macroblock rows of the band, one kind of plane.  Hand-over of the bottom sample rows:
  *   upper row -> lower row of the warp: shared-memory ring, fixed lag of one iteration (written before, read behind the
@@ -177,9 +176,9 @@ __device__ __forceinline__ void dbk_walk(const PicJob &J, DbkSmem *sm, int band,
 	uint8_t *topp = frame + (ptrdiff_t)(mby * MBW + tr) * (ptrdiff_t)stride + tpl * cpl;
 	const bool top_lane = hl < 4 && mby > 0 && row_ok;
 	const bool wb_lane = top_lane && (CH ? (hl & 1) != 0 : hl >= 1);    /* rows the top edge may change: luma -3..-1, chroma -1 */
-	volatile unsigned *prog = J.flags + W * H + (CH ? H : 0);
+	volatile unsigned *prog = row_progress(J, CH ? PROG_DBK_CHROMA : PROG_DBK_LUMA);
 	const volatile unsigned *errp = J.err;
-	const unsigned base = J.epoch * 2048u;
+	const unsigned base = prog_base(J.epoch);
 	const E264DbkMb *dgp = J.dbk + (size_t)mby * W;
 	const int pi = CH ? 1 + pl : 0;           /* plane index of alpha/beta/tc0 in row ownership */
 	uint32_t (*tile)[DBK_TS] = sm->tile[wid];
@@ -220,8 +219,7 @@ __device__ __forceinline__ void dbk_walk(const PicJob &J, DbkSmem *sm, int band,
 			const bool l_out = lrow + 2 < 2 * DBK_PAIRS && mby + 2 < H;
 			if (l_out && xl >= 1 && xl <= W) {
 				unsigned spins = 0; bool bad = false;
-				volatile int *tk = sm->taken + lrow + 2;
-				while (*tk < xl - DBK_RING && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
+				wait_smem_ge(sm->taken + lrow + 2, xl - DBK_RING, errp, spins, bad);
 				if (bad) atomicExch(J.err, 1u);
 			}
 		}
@@ -264,7 +262,7 @@ __device__ __forceinline__ void dbk_walk(const PicJob &J, DbkSmem *sm, int band,
 				dbk_line_chroma(c2, c3, s0, s1, b0, a_mb, b_mb, tc_mb[(b0 - 1) & 3]);
 				dbk_line_chroma(s2, s3, s4, s5, b2, a_in, b_in, tc_in[(b2 - 1) & 3]);
 				carry = (carry & 0x00ffffffu) | (uint32_t)c3 << 24;
-				cur[0] = dbk_pack(s0, s1, s2, s3); cur[1] = dbk_pack(s4, s5, s6, s7);
+				cur[0] = mc_pack4(s0, s1, s2, s3); cur[1] = mc_pack4(s4, s5, s6, s7);
 			} else {
 				int s[20];
 #pragma unroll
@@ -276,13 +274,13 @@ __device__ __forceinline__ void dbk_walk(const PicJob &J, DbkSmem *sm, int band,
 				dbk_line_luma<false>(s[4], s[5], s[6], s[7], s[8], s[9], s[10], s[11], b1, a_in, b_in, tc_in[(b1 - 1) & 3], false);
 				dbk_line_luma<false>(s[8], s[9], s[10], s[11], s[12], s[13], s[14], s[15], b2, a_in, b_in, tc_in[(b2 - 1) & 3], false);
 				dbk_line_luma<false>(s[12], s[13], s[14], s[15], s[16], s[17], s[18], s[19], b3, a_in, b_in, tc_in[(b3 - 1) & 3], false);
-				carry = dbk_pack(s[0], s[1], s[2], s[3]);
+				carry = mc_pack4(s[0], s[1], s[2], s[3]);
 #pragma unroll
-				for (int k = 0; k < 4; k++) cur[k % NW] = dbk_pack(s[4 + 4 * k], s[5 + 4 * k], s[6 + 4 * k], s[7 + 4 * k]);
+				for (int k = 0; k < 4; k++) cur[k % NW] = mc_pack4(s[4 + 4 * k], s[5 + 4 * k], s[6 + 4 * k], s[7 + 4 * k]);
 			}
 		}
 		/* ---- macroblock x-1 is final for this row ---- */
-		if (to_global && fin && hl == 0 && x >= 2 && (x - 1) % DBK_CHUNK == 0) { __threadfence(); prog[mby] = base + (unsigned)(x - 1); }   /* covers the stores of earlier iterations only */
+		if (to_global && fin && hl == 0 && x >= 2 && (x - 1) % DBK_CHUNK == 0) publish_row_progress(prog + mby, base, x - 1);   /* covers the stores of earlier iterations only */
 		if (fin) {
 			uint8_t *d = rowp + (x - 1) * MBW;
 			if (CH) *(uint2 *)d = make_uint2(prev[0], carry);
@@ -306,15 +304,9 @@ __device__ __forceinline__ void dbk_walk(const PicJob &J, DbkSmem *sm, int band,
 		if (lane == 0 && act && mby > 0) {      /* lane 0 belongs to the upper row: act, mby, x are the upper row's */
 			unsigned spins = 0; bool bad = false;
 			if (wid > 0) {
-				while (*done_in < x + 1 && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
+				wait_smem_ge(done_in, x + 1, errp, spins, bad);
 				__threadfence_block();
-			} else if (avail < x + 1) {
-				const unsigned need = base + (unsigned)x + 1u;
-				unsigned v = prog[mby - 1];
-				while ((int)(v - need) < 0 && !bad) { __nanosleep(40); if ((++spins & 255) == 0) bad = *errp != 0 || spins > (1u << 22); v = prog[mby - 1]; }
-				__threadfence();
-				avail = bad ? W : (int)(v - base);
-			}
+			} else if (avail < x + 1) avail = wait_row_progress(prog + mby - 1, base, x + 1, W, errp, spins, bad);
 			if (bad) atomicExch(J.err, 1u);
 		}
 		__syncwarp();
@@ -387,7 +379,7 @@ __device__ __forceinline__ void dbk_walk(const PicJob &J, DbkSmem *sm, int band,
 	}
 	/* the band's last row is stored: let the next band finish */
 	__syncwarp();
-	if (to_global && hl == 0) { __threadfence(); prog[mby] = base + (unsigned)W; }
+	if (to_global && hl == 0) publish_row_progress(prog + mby, base, W);
 }
 
 /* MINB blocks per SM = the register budget: the kernel is a chain of dependent steps (a lone warp per scheduler issues
@@ -404,7 +396,7 @@ __global__ void __launch_bounds__(DBK_PAIRS * 32, MINB) e264_deblock_kernel(PicJ
 	for (;;) {
 		__syncthreads();
 		if (threadIdx.x < 2 * DBK_PAIRS) { sm.done[threadIdx.x] = 0; sm.taken[threadIdx.x] = 0; }
-		if (threadIdx.x == 0) sm.band = (int)atomicAdd(J.tickets + 1, 1u);
+		if (threadIdx.x == 0) sm.band = (int)atomicAdd(J.tickets + TICKET_DEBLOCK, 1u);
 		__syncthreads();
 		const int t = sm.band;
 		if (t >= 2 * bands) break;

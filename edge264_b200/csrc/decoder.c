@@ -136,7 +136,7 @@ static int parse_sps(Edge264Decoder *d, BitReader *b, SPS *out) {
 	s.gaps_allowed = br_u1(b);
 	s.width_mbs = br_ue_i(b, 4096) + 1;
 	s.height_mbs = br_ue_i(b, 4096) + 1;
-	if (s.width_mbs > 1023 || s.height_mbs > 1055 || max_num_ref_frames > 16) return EBADMSG;
+	if (s.width_mbs > E264_MAX_WIDTH_MBS || s.height_mbs > 1055 || max_num_ref_frames > 16) return EBADMSG;
 	int frame_mbs_only = br_u1(b);
 	if (!frame_mbs_only) { ret = ENOTSUP; br_u1(b); }
 	s.direct_8x8_inference = br_u1(b);

@@ -13,12 +13,6 @@
 #pragma once
 #include "recon_kernels.cuh"
 #include "deblock_kernels.cuh"
-#include "mc_math.cuh"
-
-struct __align__(16) InterStage {
-	uint4 rec4[12];
-	int16_t coef[RES_COEF_MAX];
-};
 
 __device__ __forceinline__ uint32_t ldg32(const uint8_t *p) { return __ldg((const uint32_t *)p); }
 
@@ -71,17 +65,9 @@ __device__ __forceinline__ uint32_t wp_word(uint32_t a, uint32_t b, int wa, int 
 #pragma unroll
 	for (int k = 0; k < 4; k++) {
 		const int pa = (a >> (8 * k)) & 255, pb = (b >> (8 * k)) & 255;
-		const int v = ((pa * wa + pb * wb + rnd) >> sh) + o;
-		r |= (uint32_t)min(max(v, 0), 255) << (8 * k);
+		r |= (uint32_t)mc_clip255(((pa * wa + pb * wb + rnd) >> sh) + o) << (8 * k);
 	}
 	return r;
-}
-/* prediction + residual of four packed samples; res points at four int16 (8-byte aligned) */
-__device__ __forceinline__ uint32_t add_res4(uint32_t p, const int16_t *res) {
-	const uint2 rr = *(const uint2 *)res;
-	const int r0 = (short)(rr.x & 0xffff), r1 = (short)(rr.x >> 16), r2 = (short)(rr.y & 0xffff), r3 = (short)(rr.y >> 16);
-	return mc_pack4(clip255((short)((int)(p & 255) + r0)), clip255((short)((int)((p >> 8) & 255) + r1)),
-	                clip255((short)((int)((p >> 16) & 255) + r2)), clip255((short)((int)(p >> 24) + r3)));
 }
 
 /* ---- the kernel ----
@@ -165,12 +151,7 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 	WarpSmem *ws = &sm.ws[w];
 	const int nmb = J.w_mbs * J.h_mbs;
 	const int W = J.w_mbs * 16, H = J.h_mbs * 16;
-	uint8_t *dst = J.frames + (size_t)J.dst_slot * J.frame_bytes;
-	if (lane == 0) {
-		mbar_init(&sm.bars[w][0], 1); mbar_init(&sm.bars[w][1], 1);
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-	}
+	if (lane == 0) mbar_setup(sm.bars[w], 2);
 	unsigned parity[2] = {0, 0};
 	PT_DECL
 	const int nchunks = (nmb + INTER_CHUNK - 1) / INTER_CHUNK;
@@ -194,7 +175,7 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 			const E264MbRec *r = (const E264MbRec *)sm.rec4[m];
 			if (r->kind != MBK_INTER) return 0;
 			if (r->coded == 0) return 1;
-			if (lane == 0) tma_bulk_g2s(sm.coef[w][b], J.coefs + r->coef_off, (unsigned)rec_coef_count(r) * 2u, &sm.bars[w][b]);
+			coef_request(J, r, sm.coef[w][b], &sm.bars[w][b], lane);
 			return 2;
 		};
 		int what = coef_issue(w, 0);
@@ -286,17 +267,17 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 					}
 					if (what == 2) {
 						const int16_t *ry = ws->res + (by * 4 + 2 * h) * 16 + bx * 4, *rc = ws->res + 256 + h * 64 + (by * 2) * 8 + bx * 2;
-						py[0] = add_res4(py[0], ry); py[1] = add_res4(py[1], ry + 16);
-						const uint32_t a = *(const uint32_t *)rc, bb = *(const uint32_t *)(rc + 8);
-						pc = mc_pack4(clip255((short)((int)(pc & 255) + (short)(a & 0xffff))), clip255((short)((int)((pc >> 8) & 255) + (short)(a >> 16))),
-						              clip255((short)((int)((pc >> 16) & 255) + (short)(bb & 0xffff))), clip255((short)((int)(pc >> 24) + (short)(bb >> 16))));
+						const uint2 res0 = *(const uint2 *)ry, res1 = *(const uint2 *)(ry + 16);
+						py[0] = mc_add_res4(py[0], res0.x, res0.y); py[1] = mc_add_res4(py[1], res1.x, res1.y);
+						pc = mc_add_res4(pc, *(const uint32_t *)rc, *(const uint32_t *)(rc + 8));
 					}
 					*(uint32_t *)&YT(bx * 4, by * 4 + 2 * h) = py[0]; *(uint32_t *)&YT(bx * 4, by * 4 + 2 * h + 1) = py[1];
 					*(uint16_t *)&CT(h, bx * 2, by * 2) = (uint16_t)pc; *(uint16_t *)&CT(h, bx * 2, by * 2 + 1) = (uint16_t)(pc >> 16);
 				}
 				__syncwarp();
 				if (!failed) {
-					store_mb(ws, J, dst + (size_t)(mby * 16) * J.stride_y + mbx * 16, dst + J.plane_y + (size_t)(mby * 8) * J.stride_c + mbx * 8, lane);
+					uint8_t *Y, *C; mb_planes(J, mbx, mby, Y, C);
+					store_mb(ws, J, Y, C, lane);
 					if (lane == 0) J.flags[mb] = J.epoch;     /* visible to the intra kernel through the kernel boundary */
 				}
 				__syncwarp();

@@ -5,10 +5,10 @@
  * (reference: decode order edge264_slice.c:1651-1849 with the predictors of edge264_intra.c:291-765): rows can run in
  * parallel two macroblocks apart.  Round 1 ran one warp per row with a global flag, a gpu-scope fence (which also
  * invalidates L1) and reloads of the record, the residual and the row above from L2 inside every step.  Here a block owns IR_ROWS consecutive rows (two warps each: one
- * inverse-transforms up to two macroblocks ahead, one predicts); the bottom
+ * inverse-transforms up to IR_SLOTS - 1 macroblocks ahead, one predicts); the bottom
  * sample row of every finished macroblock goes to the row below through a shared-memory ring with done/taken counters
- * (block-scope fences); records arrive two macroblocks ahead, coefficient runs one ahead (cp.async.bulk on an mbarrier) and
- * are inverse-transformed BEFORE the row waits for its neighbours, so a step is the prediction itself plus a
+ * (block-scope fences); records arrive four macroblocks ahead, coefficient runs three ahead (cp.async.bulk on an mbarrier)
+ * and are inverse-transformed BEFORE the row waits for its neighbours, so a step is the prediction itself plus a
  * shared-memory hand-shake and the residual never travels through global memory.  Only the band's last row talks to the next block through global memory, with
  * a progress counter published every IR_CHUNK macroblocks.  Inter macroblocks inside such a picture were reconstructed
  * by the inter kernel before: their row warp only forwards their border samples. */
@@ -22,7 +22,7 @@
 #define IR_SLOTS 4      /* macroblocks the transform warp may be ahead of the prediction warp (residual / tile slots, coefficient buffers) */
 #define IR_RECS 8       /* record ring of a row */
 struct __align__(16) IntraRowsSmem {
-	WarpSmem ws[IR_ROWS][IR_SLOTS];                    /* macroblocks x and x+1 of every row: residual from the row's transform warp, tile of its prediction warp */
+	WarpSmem ws[IR_ROWS][IR_SLOTS];                    /* macroblock x of every row in slot x % IR_SLOTS: residual from the row's transform warp, tile of its prediction warp */
 	uint4 recs[IR_ROWS][IR_RECS][12];           /* records of macroblocks x-4 .. x+3 of every row */
 	uint32_t ring[IR_ROWS][IR_RING][8];         /* bottom sample row of a finished macroblock: luma (4 words), Cb (2), Cr (2) */
 	int16_t coef[IR_ROWS][IR_SLOTS][RES_COEF_MAX];   /* coefficient runs of macroblocks x .. x+3 of every row (cp.async.bulk) */
@@ -58,7 +58,7 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 	auto coef_issue = [&](int x) -> bool {       /* true: a copy is in flight into buffer x % IR_SLOTS */
 		const E264MbRec *rr = (const E264MbRec *)sm.recs[w][x % IR_RECS];
 		if (rr->kind == MBK_INTER || rr->kind == MBK_IPCM || rr->coded == 0) return false;
-		if (lane == 0) tma_bulk_g2s(sm.coef[w][x % IR_SLOTS], J.coefs + rr->coef_off, (unsigned)rec_coef_count(rr) * 2u, &sm.bars[w][x % IR_SLOTS]);
+		coef_request(J, rr, sm.coef[w][x % IR_SLOTS], &sm.bars[w][x % IR_SLOTS], lane);
 		return true;
 	};
 	unsigned pending = 0;                        /* bit x % IR_SLOTS: macroblock x has a copy in flight */
@@ -73,7 +73,7 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 		 * below belonged to macroblock mbx + AHEAD + 1 - IR_RECS, older still */
 		if (lane == 0) {
 			unsigned spins = 0; bool bad = false;
-			while (*used < mbx - IR_SLOTS + 1 && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
+			wait_smem_ge(used, mbx - IR_SLOTS + 1, errp, spins, bad);
 			if (bad) atomicExch(J.err, 1u);
 			__threadfence_block();
 		}
@@ -93,10 +93,7 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 			parbits ^= 1u << sl;
 			PT_MARK(2)  /* waiting for the coefficient run */
 			residual_stage(ws, r, J.slices + r->slice_idx, sm.coef[w][sl], lane);
-		} else if (kind != MBK_INTER && kind != MBK_IPCM) {
-			((uint4 *)ws->res)[lane] = make_uint4(0, 0, 0, 0);
-			if (lane < 16) ((uint4 *)ws->res)[32 + lane] = make_uint4(0, 0, 0, 0);
-		}
+		} else if (kind != MBK_INTER && kind != MBK_IPCM) clear_residual(ws, lane);
 		__syncwarp();
 		if (lane == 0) { __threadfence_block(); *ready = mbx + 1; }
 		PT_MARK(3)      /* inverse transforms */
@@ -112,48 +109,40 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 }
 
 /* The row's PREDICTION warp: waits for the residual, for the row above (top-right neighbour finished) and for room in
- * its ring, predicts into the tile of slot x & 1, stores, hands the bottom sample row down. */
+ * its ring, predicts into the tile of slot x % IR_SLOTS, stores, hands the bottom sample row down. */
 __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &sm, int band, int w, int lane) {
-	const int W = J.w_mbs, H = J.h_mbs, nmb = W * H;
+	const int W = J.w_mbs, H = J.h_mbs;
 	const int lrow = w, mby = band * IR_ROWS + w;
 	if (mby >= H) return;
 	const bool from_global = lrow == 0 && mby > 0;
 	const bool from_ring = lrow > 0;
 	const bool to_ring = lrow + 1 < IR_ROWS && mby + 1 < H;
 	const bool to_global = lrow + 1 == IR_ROWS && mby + 1 < H;
-	volatile unsigned *prog = J.flags + nmb + 2 * H;          /* intra row progress (third counter array) */
+	volatile unsigned *prog = row_progress(J, PROG_INTRA);
 	const volatile unsigned *errp = J.err;
-	const unsigned base = J.epoch * 2048u;
+	const unsigned base = prog_base(J.epoch);
 	volatile int *done_in = sm.done + (lrow > 0 ? lrow - 1 : 0), *done_out = sm.done + lrow;
 	volatile int *taken_me = sm.taken + lrow, *taken_next = sm.taken + (lrow + 1 < IR_ROWS ? lrow + 1 : lrow);
 	volatile int *ready = sm.ready + w, *used = sm.used + w;
 	uint32_t (*ring_in)[8] = sm.ring[lrow > 0 ? lrow - 1 : 0];
 	uint32_t (*ring_out)[8] = sm.ring[lrow];
-	uint8_t *dst = J.frames + (size_t)J.dst_slot * J.frame_bytes;
 	const int cpl = J.stride_c >> 1;
 	int avail = 0;                                            /* macroblocks of the row above the band known to be stored */
 	PT_DECL
 #pragma unroll 1
 	for (int mbx = 0; mbx < W; mbx++) {
-		uint8_t *Y = dst + (size_t)(mby * 16) * J.stride_y + mbx * 16;
-		uint8_t *C = dst + J.plane_y + (size_t)(mby * 8) * J.stride_c + mbx * 8;
+		uint8_t *Y, *C; mb_planes(J, mbx, mby, Y, C);
 		/* ---- wait: residual delivered; row above through with macroblocks up to x+1 (top-right neighbour); room in our ring ---- */
 		if (lane == 0) {
 			unsigned spins = 0; bool bad = false;
-			while (*ready <= mbx && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
+			wait_smem_ge(ready, mbx + 1, errp, spins, bad);
 			PT_MARK(0)  /* waiting for the residual */
 			const int need = min(mbx + 2, W);
-			if (from_ring) {
-				while (*done_in < need && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
-			} else if (from_global && avail < need) {
-				const unsigned target = base + (unsigned)need;
-				unsigned v = prog[mby - 1];
-				while ((int)(v - target) < 0 && !bad) { __nanosleep(40); if ((++spins & 255) == 0) bad = *errp != 0 || spins > (1u << 22); v = prog[mby - 1]; }
-				__threadfence();
-				avail = bad ? W : (int)(v - base);
-			}
+			if (from_ring) wait_smem_ge(done_in, need, errp, spins, bad);
+			else if (from_global && avail < need) avail = wait_row_progress(prog + mby - 1, base, need, W, errp, spins, bad);
 			PT_MARK(1)  /* waiting for the row above */
-			if (to_ring) while (*taken_next <= mbx - IR_RING + 1 && !bad)     /* entry mbx - RING is still the corner sample of the row below's macroblock mbx - RING + 1 */ { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > (1u << 26); }
+			/* entry mbx - RING is still the corner sample of the row below's macroblock mbx - RING + 1 */
+			if (to_ring) wait_smem_ge(taken_next, mbx - IR_RING + 2, errp, spins, bad);
 			if (bad) atomicExch(J.err, 1u);
 			__threadfence_block();
 			*taken_me = mbx;
@@ -170,11 +159,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 			else if (lane >= 8 && lane < 12) *(uint32_t *)&CT((lane - 8) >> 1, 4 * (lane & 1), -1) = ring_in[mbx % IR_RING][lane - 4];
 			else if (lane == 12) { if (mbx > 0) CT(0, -1, -1) = (uint8_t)(ring_in[(mbx - 1) % IR_RING][5] >> 24); }
 			else if (lane == 13) { if (mbx > 0) CT(1, -1, -1) = (uint8_t)(ring_in[(mbx - 1) % IR_RING][7] >> 24); }
-		} else if (from_global) {
-			const int x = lane - 1;   /* -1..23 */
-			if (x < 24 && (x >= 0 || mbx > 0) && (x < 16 || mbx < W - 1)) YT(x, -1) = __ldcg(Y - J.stride_y + x);
-			if (lane < 18) { const int pl = lane / 9, cx = lane % 9 - 1; if (cx >= 0 || mbx > 0) CT(pl, cx, -1) = __ldcg(C + pl * cpl - J.stride_c + cx); }
-		}
+		} else if (from_global) load_row_above(ws, Y - J.stride_y, C - J.stride_c, cpl, mbx > 0, mbx < W - 1, lane);
 		__syncwarp();
 		PT_MARK(2)      /* ring room, hand-shake, row above into the tile */
 		/* ---- the macroblock ---- */
@@ -186,12 +171,8 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 				else if (lane < 8) ring_out[mbx % IR_RING][lane] = __ldcg((const uint32_t *)(C + ((lane - 4) >> 1) * cpl + (size_t)7 * J.stride_c) + (lane & 1));
 			}
 		} else {
-			if (kind == MBK_IPCM) {
-				const uint8_t *s = (const uint8_t *)(J.coefs + r->coef_off);
-				if (lane < 16) *(uint4 *)&YT(0, lane) = __ldg((const uint4 *)s + lane);
-				else { const int j = lane - 16; *(uint2 *)&CT(j >> 3, 0, j & 7) = __ldg((const uint2 *)(s + 256) + j); }
-				__syncwarp();
-			} else {
+			if (kind == MBK_IPCM) load_pcm(ws, J, r, lane);
+			else {
 				intra_luma(ws, r, lane);
 				PT_MARK(3)  /* luma prediction */
 				intra_chroma(ws, r, lane);
@@ -208,7 +189,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 		/* ---- publish: shared-memory counter for the row below in this band; global counter for the next band, one chunk late ---- */
 		if (lane == 0) {
 			if (to_ring) { __threadfence_block(); *done_out = mbx + 1; }
-			if (to_global && mbx > 0 && mbx % IR_CHUNK == 0) { __threadfence(); prog[mby] = base + (unsigned)mbx; }   /* covers macroblocks 0..mbx-1, stored in earlier iterations */
+			if (to_global && mbx > 0 && mbx % IR_CHUNK == 0) publish_row_progress(prog + mby, base, mbx);   /* covers macroblocks 0..mbx-1, stored in earlier iterations */
 		}
 		/* right-most column becomes the next macroblock's left neighbour (the other slot's tile) */
 		{
@@ -226,7 +207,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 	__syncwarp();
 	if (lane == 0) {
 		*taken_me = W + IR_RING;       /* nothing of the ring above is needed any more */
-		if (to_global) { __threadfence(); prog[mby] = base + (unsigned)W; }
+		if (to_global) publish_row_progress(prog + mby, base, W);
 	}
 }
 
@@ -239,16 +220,12 @@ __global__ void __launch_bounds__(IR_ROWS * 64) e264_intra_rows_kernel(PicJob J)
 	const bool transform = wid >= IR_ROWS;
 	const int bands = (J.h_mbs + IR_ROWS - 1) / IR_ROWS;
 	unsigned parbits = 0;
-	if (transform && lane == 0) {
-		for (int k = 0; k < IR_SLOTS; k++) mbar_init(&sm.bars[w][k], 1);
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-	}
+	if (transform && lane == 0) mbar_setup(sm.bars[w], IR_SLOTS);
 	/* bands in dispatch order: a band only waits for bands drawn before it */
 	for (;;) {
 		__syncthreads();
 		if (threadIdx.x < IR_ROWS) { sm.done[threadIdx.x] = 0; sm.taken[threadIdx.x] = 0; sm.ready[threadIdx.x] = 0; sm.used[threadIdx.x] = 0; }
-		if (threadIdx.x == 0) sm.band = (int)atomicAdd(J.tickets + 2, 1u);
+		if (threadIdx.x == 0) sm.band = (int)atomicAdd(J.tickets + TICKET_INTRA, 1u);
 		__syncthreads();
 		const int band = sm.band;
 		if (band >= bands) break;
@@ -283,17 +260,12 @@ __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) 
 	const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 	WarpSmem *ws = &sm.ws[w];
 	const int nmb = J.w_mbs * J.h_mbs, W = J.w_mbs, cpl = J.stride_c >> 1;
-	uint8_t *dst = J.frames + (size_t)J.dst_slot * J.frame_bytes;
 	unsigned parity = 0;
-	if (lane == 0) {
-		mbar_init(&sm.bars[w], 1);
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-	}
+	if (lane == 0) mbar_setup(&sm.bars[w], 1);
 	__syncwarp();
 	for (;;) {
 		unsigned t = 0;
-		if (lane == 0) t = atomicAdd(J.tickets + 2, 1u);
+		if (lane == 0) t = atomicAdd(J.tickets + TICKET_INTRA, 1u);
 		t = __shfl_sync(0xffffffffu, t, 0);
 		if (t >= (unsigned)J.n_intra) break;
 		const int mb = (int)__ldg(J.intra_list + t);
@@ -304,25 +276,17 @@ __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) 
 		const E264MbRec *r = (const E264MbRec *)ws->rec4;
 		const int kind = r->kind;
 		if (kind == MBK_INTER) continue;      /* (the list holds intra macroblocks only) */
-		uint8_t *Y = dst + (size_t)(mby * 16) * J.stride_y + mbx * 16;
-		uint8_t *C = dst + J.plane_y + (size_t)(mby * 8) * J.stride_c + mbx * 8;
+		uint8_t *Y, *C; mb_planes(J, mbx, mby, Y, C);
 		if (kind == MBK_IPCM) {
-			const uint8_t *s = (const uint8_t *)(J.coefs + r->coef_off);
-			if (lane < 16) *(uint4 *)&YT(0, lane) = __ldg((const uint4 *)s + lane);
-			else { const int j = lane - 16; *(uint2 *)&CT(j >> 3, 0, j & 7) = __ldg((const uint2 *)(s + 256) + j); }
-			__syncwarp();
+			load_pcm(ws, J, r, lane);
 			store_mb(ws, J, Y, C, lane);
 		} else {
-			const bool coded = r->coded != 0;
-			if (coded && lane == 0) tma_bulk_g2s(sm.coef[w], J.coefs + r->coef_off, (unsigned)rec_coef_count(r) * 2u, &sm.bars[w]);
-			if (coded) {
+			if (r->coded != 0) {
+				coef_request(J, r, sm.coef[w], &sm.bars[w], lane);
 				if (!mbar_wait(&sm.bars[w], parity)) { if (lane == 0) atomicExch(J.err, 3u); }
 				parity ^= 1;
 				residual_stage(ws, r, J.slices + r->slice_idx, sm.coef[w], lane);
-			} else {
-				((uint4 *)ws->res)[lane] = make_uint4(0, 0, 0, 0);
-				if (lane < 16) ((uint4 *)ws->res)[32 + lane] = make_uint4(0, 0, 0, 0);
-			}
+			} else clear_residual(ws, lane);
 			{	/* A, D, B, C: one lane each, the four round trips overlap */
 				int idx = -1;
 				if (lane == 0 && mbx > 0) idx = mb - 1;
@@ -332,11 +296,7 @@ __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) 
 				if (idx >= 0) wait_flag_acquire(J.flags, idx, J.epoch, J.err);
 			}
 			__syncwarp();
-			if (mby > 0) {
-				const int x = lane - 1;   /* -1..23 */
-				if (x < 24 && (x >= 0 || mbx > 0) && (x < 16 || mbx < W - 1)) YT(x, -1) = __ldcg(Y - J.stride_y + x);
-				if (lane < 18) { const int pl = lane / 9, cx = lane % 9 - 1; if (cx >= 0 || mbx > 0) CT(pl, cx, -1) = __ldcg(C + pl * cpl - J.stride_c + cx); }
-			}
+			if (mby > 0) load_row_above(ws, Y - J.stride_y, C - J.stride_c, cpl, mbx > 0, mbx < W - 1, lane);
 			if (mbx > 0) {
 				if (lane < 16) YT(-1, lane) = __ldcg(Y + (size_t)lane * J.stride_y - 1);
 				else { const int j = lane - 16, pl = j >> 3, row = j & 7; CT(pl, -1, row) = __ldcg(C + pl * cpl + (size_t)row * J.stride_c - 1); }

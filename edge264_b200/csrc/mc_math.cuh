@@ -30,6 +30,12 @@ MC_FN uint32_t mc_prmt(uint32_t a, uint32_t b, uint32_t sel) {
 
 MC_FN int mc_clip255(int v) { return v < 0 ? 0 : v > 255 ? 255 : v; }
 MC_FN uint32_t mc_pack4(int a, int b, int c, int d) { return (uint32_t)a | (uint32_t)b << 8 | (uint32_t)c << 16 | (uint32_t)d << 24; }
+/* four predicted samples (bytes of p) plus four int16 residuals (r01: the first two, r23: the last two), clipped; the sum
+ * wraps to 16 bits first like the reference's 16-bit adds (residuals of conforming streams never make it wrap) */
+MC_FN uint32_t mc_add_res4(uint32_t p, uint32_t r01, uint32_t r23) {
+	return mc_pack4(mc_clip255((int16_t)((int)(p & 255u) + (int16_t)(r01 & 0xffffu))), mc_clip255((int16_t)((int)((p >> 8) & 255u) + (int16_t)(r01 >> 16))),
+	                mc_clip255((int16_t)((int)((p >> 16) & 255u) + (int16_t)(r23 & 0xffffu))), mc_clip255((int16_t)((int)(p >> 24) + (int16_t)(r23 >> 16))));
+}
 /* rounded-up average of four bytes at once */
 MC_FN uint32_t mc_avg4(uint32_t a, uint32_t b) { return (a | b) - (((a ^ b) >> 1) & 0x7f7f7f7fu); }
 

@@ -3,7 +3,7 @@
  * Replaces the reference's in-process contract between the slice parser and the pixel functions
  * (reference: prototypes edge264_internal.h:1349-1374, call sites edge264_slice.c:466-664,881,1816,
  * edge264_mvpred.c:73-513, edge264_headers.c:510,551) by: pinned staging filled by the parser ->
- * cudaMemcpyAsync -> two kernels per picture on the decoder's stream -> cudaMemcpyAsync of the
+ * cudaMemcpyAsync -> up to three kernels per picture on the decoder's stream -> cudaMemcpyAsync of the
  * finished frame into a pinned host mirror.  Frames live in HBM in the reference's own layout
  * (edge264_headers.c:2027-2046) so the mirror is what edge264_get_frame hands out.
  * There is NO CPU fallback: without a CUDA device e264b_create() fails and edge264_alloc() returns NULL.
@@ -43,7 +43,7 @@ struct E264bDevice {
 	uint8_t *d_frames;
 	E264MbRec *h_recs[E264_MAX_SLOTS]; cudaEvent_t rec_up[E264_MAX_SLOTS]; bool rec_busy[E264_MAX_SLOTS];
 	Staging st[NSTAGE]; int stage, n_stage;
-	unsigned *d_sync;            /* [0..7] tickets (0 inter, 1 deblock, 2 intra), [8] err, [16..) flags[nmb] + row progress[3 * h_mbs] */
+	unsigned *d_sync;            /* synchronisation words, layout SYNC_* in recon_kernels.cuh */
 	size_t sync_words;
 	unsigned epoch;
 	cudaEvent_t tick_ev[NTICK]; uint64_t tick_seq;
@@ -180,7 +180,7 @@ extern "C" int e264b_configure(E264bDevice *c, const E264PicDesc *g, int n_slots
 		CK(cudaMalloc(&s->d_intra, c->nmb * sizeof(uint32_t)));
 		CK(cudaHostAlloc(&s->h_intra, c->nmb * sizeof(uint32_t), cudaHostAllocDefault));
 	}
-	c->sync_words = 16 + c->nmb + 3 * (size_t)g->height_mbs + 16;
+	c->sync_words = SYNC_FLAGS + c->nmb + PROG_ARRAYS * (size_t)g->height_mbs + 16;
 	CK(cudaMalloc(&c->d_sync, c->sync_words * sizeof(unsigned)));
 	CK(cudaMemsetAsync(c->d_sync, 0, c->sync_words * sizeof(unsigned), c->stream));
 	c->epoch = 0; c->stage = 0;
@@ -227,18 +227,18 @@ static PicJob make_job(E264bDevice *c, const E264PicDesc *pd, int stage, const E
 	J.recs = recs; J.coefs = coefs; J.slices = slices; J.frames = c->d_frames;
 	J.frame_bytes = pd->frame_bytes; J.w_mbs = pd->width_mbs; J.h_mbs = pd->height_mbs;
 	J.stride_y = pd->stride_y; J.stride_c = pd->stride_c; J.plane_y = pd->plane_y; J.dst_slot = pd->dst_slot; J.n_slots = c->n_slots;
-	J.err = c->d_sync + 8; J.flags = c->d_sync + 16;
+	J.err = c->d_sync + SYNC_ERR; J.flags = c->d_sync + SYNC_FLAGS;
 	J.dbk = pd->any_deblock ? c->st[stage].d_dbk : NULL;
 	J.intra_list = intra; J.n_intra = pd->n_intra;
 	J.rows_mode = pd->n_intra * 2 > pd->width_mbs * pd->height_mbs;   /* intra pictures: wavefront of row warps */
 	J.trace = NULL; J.trace_base = 0; J.trace_rep = NULL; J.trace_rep_stride = 0; J.diag = 0;
-	if (c->epoch >= (1u << 20)) {   /* row progress counters encode epoch * 2048 + count: restart before it wraps */
+	if (c->epoch >= PROG_MAX_EPOCH) {   /* restart before the row-progress words leave the range their waits compare in */
 		cudaStreamSynchronize(c->stream);
 		cudaMemsetAsync(c->d_sync, 0, c->sync_words * sizeof(unsigned), c->stream);
 		c->epoch = 0;
 	}
 	J.epoch = ++c->epoch;
-	J.tickets = c->d_sync + (J.epoch & 1) * 4; J.tickets_next = c->d_sync + ((J.epoch + 1) & 1) * 4;    /* two sets, pictures alternate; every kernel clears the next picture's */
+	J.tickets = c->d_sync + SYNC_TICKETS + (J.epoch & 1) * 4; J.tickets_next = c->d_sync + SYNC_TICKETS + ((J.epoch + 1) & 1) * 4;    /* two sets, pictures alternate; every kernel clears the next picture's */
 	return J;
 }
 static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd, int with_deblock) {
@@ -311,7 +311,7 @@ extern "C" int e264b_submit(E264bDevice *c, const E264PicDesc *pd, uint8_t *host
 		static int dbg = -1; if (dbg < 0) { const char *e = getenv("E264B_DEBUG_SYNC"); dbg = e ? atoi(e) : 0; }
 		if (dbg) {
 			fprintf(stderr, "e264b: picture slot %d epoch %u (intra %d of %d, coefs %u) launched, waiting...\n", pd->dst_slot, J.epoch, pd->n_intra, J.w_mbs * J.h_mbs, pd->n_coefs);
-			cudaError_t e = cudaStreamSynchronize(c->stream); unsigned v = 0; cudaMemcpy(&v, c->d_sync + 8, sizeof(v), cudaMemcpyDeviceToHost);
+			cudaError_t e = cudaStreamSynchronize(c->stream); unsigned v = 0; cudaMemcpy(&v, c->d_sync + SYNC_ERR, sizeof(v), cudaMemcpyDeviceToHost);
 			fprintf(stderr, "e264b:   -> %s, device error word %u\n", cudaGetErrorString(e), v);
 		}
 	}
@@ -330,7 +330,7 @@ extern "C" int e264b_submit(E264bDevice *c, const E264PicDesc *pd, uint8_t *host
 	}
 	CK(cudaEventRecord(s->done, c->stream)); s->busy = true;
 	uint64_t t = ++c->tick_seq;
-	if (c->d_sync) CK(cudaMemcpyAsync(&c->h_err[t % NTICK], c->d_sync + 8, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+	if (c->d_sync) CK(cudaMemcpyAsync(&c->h_err[t % NTICK], c->d_sync + SYNC_ERR, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
 	CK(cudaEventRecord(c->tick_ev[t % NTICK], c->stream));
 	*ticket = t;
 	return 0;
@@ -371,7 +371,7 @@ extern "C" int e264b_error_flag(E264bDevice *c) {
 	unsigned v = 0;
 	cudaSetDevice(c->dev);
 	cudaStreamSynchronize(c->stream);
-	cudaMemcpy(&v, c->d_sync + 8, sizeof(v), cudaMemcpyDeviceToHost);
+	cudaMemcpy(&v, c->d_sync + SYNC_ERR, sizeof(v), cudaMemcpyDeviceToHost);
 	return (int)v;
 }
 extern "C" void e264b_stats(E264bDevice *c, uint64_t *launches, uint64_t *h2d, uint64_t *d2h) { if (launches) *launches = c->launches; if (h2d) *h2d = c->h2d_bytes; if (d2h) *d2h = c->d2h_bytes; }

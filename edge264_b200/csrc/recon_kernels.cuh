@@ -13,18 +13,31 @@
 #include <stdint.h>
 #include "records.h"
 #include "h264_tables.h"
+#include "mc_math.cuh"
+
+/* Synchronisation words of a decoder (recon.cu): two sets of 4 tickets (TICKET_*; pictures alternate), the error word
+ * (1 a dependency wait gave up, 3 / 4 an intra / inter coefficient copy did not arrive), then [nmb] "reconstructed" flags
+ * (== epoch) and PROG_ARRAYS arrays of h_mbs row-progress words (epoch * PROG_STRIDE + macroblocks done): nothing is
+ * cleared between pictures.  The progress waits compare signed differences, so the host restarts the epochs at
+ * PROG_MAX_EPOCH. */
+enum { SYNC_TICKETS = 0, SYNC_ERR = 8, SYNC_FLAGS = 16 };
+enum { TICKET_DEBLOCK = 1, TICKET_INTRA = 2 };
+enum { PROG_DBK_LUMA = 0, PROG_DBK_CHROMA = 1, PROG_INTRA = 2, PROG_ARRAYS = 3 };
+#define PROG_STRIDE 2048u
+#define PROG_MAX_EPOCH (0x80000000u / PROG_STRIDE)
+static_assert(E264_MAX_WIDTH_MBS < PROG_STRIDE, "a row's progress count must stay below the epoch stride");
 
 struct PicJob {
 	const E264MbRec *recs; const int16_t *coefs; const E264SliceRec *slices;
 	uint8_t *frames;
 	int frame_bytes, w_mbs, h_mbs, stride_y, stride_c, plane_y, dst_slot, n_slots;
-	unsigned *flags;      /* [nmb] "reconstructed" == epoch, then [3][h_mbs] row progress (epoch * 2048 + macroblocks done): deblocking luma, deblocking chroma, intra pictures */
+	unsigned *flags;      /* [SYNC_FLAGS ..] of the synchronisation words */
 	unsigned epoch;
-	unsigned *tickets;    /* [4] this picture's ticket words: 1 deblock bands, 2 intra list / intra bands */
+	unsigned *tickets;    /* [4] this picture's ticket words (TICKET_*) */
 	unsigned *tickets_next;   /* [4] the next picture's: every kernel clears them on entry (pictures alternate between two sets, so no memset and no extra launch separates two pictures) */
 	unsigned *err;
 	int rows_mode;
-	struct E264DbkMb *dbk;        /* [nmb] deblocking digests written by e264_prepass_kernel; NULL = picture is not deblocked */
+	struct E264DbkMb *dbk;        /* [nmb] deblocking digests written by the inter kernel (the intra-rows kernel in pictures without inter macroblocks); NULL = picture is not deblocked */
 	const uint32_t *intra_list;   /* addresses of the intra macroblocks in raster order */
 	int n_intra;
 	unsigned long long *trace;   /* measurement only (e264b_replay): [trace_base + kind] = {first block start, last block end} in globaltimer ns; kinds: 1 inter, 2 intra, 3 deblock */
@@ -34,7 +47,6 @@ struct PicJob {
 	int diag;                    /* measurement only: count block placement per SM (g_diag_*) */
 };
 
-#define WARPS_PER_BLOCK 4
 #define YT_STRIDE 48     /* luma tile row: [15]=left neighbour, [16..31]=samples, [32..39]=top-right */
 #define CT_STRIDE 16     /* chroma tile row: [7]=left neighbour, [8..15]=samples */
 struct __align__(16) WarpSmem {
@@ -49,12 +61,10 @@ struct __align__(16) WarpSmem {
 	} u;
 };
 
-__device__ __forceinline__ int clip255(int v) { return min(max(v, 0), 255); }
 __device__ __forceinline__ int sat16(int v) { return min(max(v, -32768), 32767); }
 __device__ __forceinline__ int blk_x(int b) { return (b & 1) | ((b >> 1) & 2); }
 __device__ __forceinline__ int blk_y(int b) { return ((b >> 1) & 1) | ((b >> 2) & 2); }
 __device__ __forceinline__ int blk_z(int x, int y) { return (x & 1) | ((y & 1) << 1) | ((x & 2) << 1) | ((y & 2) << 2); }
-__device__ __forceinline__ int norm4(int m, int i, int j) { return h264_norm4x4[m][((i & 1) && (j & 1)) ? 1 : (!(i & 1) && !(j & 1)) ? 0 : 2]; }
 __device__ __forceinline__ void reset_next_tickets(const PicJob &J) { if (blockIdx.x == 0 && threadIdx.x < 4) J.tickets_next[threadIdx.x] = 0; }
 
 /* measurement only (replay with E264B_DIAG=1): how the blocks of each kernel kind land on the SMs —
@@ -83,10 +93,10 @@ struct TraceScope {
 	__device__ __forceinline__ ~TraceScope() { if (t && threadIdx.x == 0) atomicMax(t + 1, now()); if (dk >= 0 && threadIdx.x == 0) atomicSub(&g_diag_cur[dk][sm], 1u); }
 };
 
-/* Dependency waits are bounded so that a bug cannot hang the GPU: they give up after ~0.2 s of SM clocks, or at once when
- * another warp has already raised the error flag. */
-/* spin until flags[idx] == epoch, with acquire loads (no fence behind it): several lanes of a warp may each wait for their
- * own flag, so the round trips to L2 overlap instead of adding up; a __syncwarp() behind the waits orders the other lanes' loads */
+/* Dependency waits are bounded so that a bug cannot hang the GPU: they give up after a budget, or at once when another
+ * warp has already raised the error flag.  wait_flag_acquire spins (~0.2 s of SM clocks) until flags[idx] == epoch, with
+ * acquire loads (no fence behind it): several lanes of a warp may each wait for their own flag, so the round trips to L2
+ * overlap instead of adding up; a __syncwarp() behind the waits orders the other lanes' loads */
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) { unsigned v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ bool wait_flag_acquire(const unsigned *flags, int idx, unsigned epoch, unsigned *err) {
 	const unsigned *f = flags + idx;
@@ -103,6 +113,27 @@ __device__ __forceinline__ bool wait_flag_acquire(const unsigned *flags, int idx
 	}
 	return ok;
 }
+/* The waits of the wavefront kernels, by ONE lane: single-exit loops, so the warp reconverges at the caller's __syncwarp().
+ * `spins` and `bad` are the caller's (several waits in a row spend one budget); the caller raises the error word. */
+#define SMEM_SPIN_BUDGET (1u << 26)   /* shared-memory polls */
+#define PROG_SPIN_BUDGET (1u << 22)   /* global row-progress polls, 40 ns apart */
+/* until the shared-memory counter *c reaches target */
+__device__ __forceinline__ void wait_smem_ge(const volatile int *c, int target, const volatile unsigned *errp, unsigned &spins, bool &bad) {
+	while (*c < target && !bad) { if ((++spins & 1023) == 0) bad = *errp != 0 || spins > SMEM_SPIN_BUDGET; }
+}
+__device__ __forceinline__ volatile unsigned *row_progress(const PicJob &J, int array) { return J.flags + J.w_mbs * J.h_mbs + array * J.h_mbs; }
+__device__ __forceinline__ unsigned prog_base(unsigned epoch) { return epoch * PROG_STRIDE; }
+/* until row-progress word *p covers `need` macroblocks of this epoch (base = prog_base(epoch)); then a gpu-scope fence.
+ * Returns the macroblocks of that row known to be stored: w (the row's width) once the wait has given up. */
+__device__ __forceinline__ int wait_row_progress(const volatile unsigned *p, unsigned base, int need, int w, const volatile unsigned *errp, unsigned &spins, bool &bad) {
+	const unsigned target = base + (unsigned)need;
+	unsigned v = *p;
+	while ((int)(v - target) < 0 && !bad) { __nanosleep(40); if ((++spins & 255) == 0) bad = *errp != 0 || spins > PROG_SPIN_BUDGET; v = *p; }
+	__threadfence();
+	return bad ? w : (int)(v - base);
+}
+/* macroblocks 0 .. n-1 of the row are stored: a gpu-scope fence, then the word */
+__device__ __forceinline__ void publish_row_progress(volatile unsigned *p, unsigned base, int n) { __threadfence(); *p = base + (unsigned)n; }
 /* ---- shared-memory barrier + TMA helpers (sm_90+ PTX; SASS: SYNCS.*, UBLKCP, UTMALDG) ---- */
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(void *bar, unsigned count) {
@@ -112,6 +143,12 @@ __device__ __forceinline__ void tma_bulk_g2s(void *dst, const void *src, unsigne
 	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
 	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
 	             :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+/* by one lane: n barriers of one arrival each, made visible to the async proxy that completes them */
+__device__ __forceinline__ void mbar_setup(unsigned long long *bars, int n) {
+	for (int k = 0; k < n; k++) mbar_init(&bars[k], 1);
+	asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 /* wait for the phase with the given parity; gives up after ~10 ms of SM clocks (a window arrives in
  * microseconds), false = gave up (the caller raises the error flag).  One loop, one exit: ptxas reconverges the
@@ -188,12 +225,15 @@ __device__ __forceinline__ void idct8_1d(short a[8]) {
 	a[4] = (short)(f6 - f1); a[5] = (short)(f4 - f3); a[6] = (short)(f2 - f5); a[7] = (short)(f0 - f7);
 }
 
+/* the whole residual to zero (768 bytes, one or two 16-byte stores per lane) */
+__device__ __forceinline__ void clear_residual(WarpSmem *ws, int lane) {
+	((uint4 *)ws->res)[lane] = make_uint4(0, 0, 0, 0);
+	if (lane < 16) ((uint4 *)ws->res)[32 + lane] = make_uint4(0, 0, 0, 0);
+}
+
 /* cf: this macroblock's coefficient run, staged in shared memory by the caller (cp.async.bulk) */
 __device__ __noinline__ void residual_stage(WarpSmem *ws, const E264MbRec *r, const E264SliceRec *sr, const int16_t *cf, int lane) {
-	/* clear */
-	uint4 z = make_uint4(0, 0, 0, 0);
-	((uint4 *)ws->res)[lane] = z;
-	if (lane < 16) ((uint4 *)ws->res)[32 + lane] = z;
+	clear_residual(ws, lane);
 	const unsigned coded = r->coded;
 	const int inter = r->kind == MBK_INTER, i16 = r->kind == MBK_I16x16;
 	const int qpy = r->qp[0];
@@ -387,14 +427,6 @@ __device__ __forceinline__ void pred8x8_warp(const WarpSmem *ws, int X0, int Y0,
 	v1 = intra_tap_apply(E, e1 & 31, e1 >> 5);
 }
 
-/* four predicted samples (bytes of p) plus four int16 residuals (r01 = first two, r23 = last two), clipped to 8 bits;
- * the sum wraps in 16 bits first like the reference's saturating 16-bit adds never see it: v + res fits unless res is garbage */
-__device__ __forceinline__ uint32_t intra_add_res4(uint32_t p, uint32_t r01, uint32_t r23) {
-	const int v0 = clip255((short)((int)(p & 255u) + (short)(r01 & 0xffffu))), v1 = clip255((short)((int)((p >> 8) & 255u) + (short)(r01 >> 16)));
-	const int v2 = clip255((short)((int)((p >> 16) & 255u) + (short)(r23 & 0xffffu))), v3 = clip255((short)((int)(p >> 24) + (short)(r23 >> 16)));
-	return (uint32_t)v0 | (uint32_t)v1 << 8 | (uint32_t)v2 << 16 | (uint32_t)v3 << 24;
-}
-
 __device__ __noinline__ void intra_luma(WarpSmem *ws, const E264MbRec *r, int lane) {
 	if (r->kind == MBK_I4x4) {
 		/* the 16 blocks along anti-diagonals: block (x, y) in step x + 2 y, so its left, top, top-left and top-right
@@ -408,7 +440,7 @@ __device__ __noinline__ void intra_luma(WarpSmem *ws, const E264MbRec *r, int la
 			const bool on = bx >= 0 && bx < 4 && by < 4;
 			const int X0 = on ? bx * 4 : 0, Y0 = on ? by * 4 : 0;
 			int v = pred4x4_half(ws, X0, Y0, r->modes[on ? blk_z(bx, by) : 0], taps, hl, half);
-			v = clip255((short)(v + ws->res[(Y0 + y) * 16 + X0 + x]));
+			v = mc_clip255((int16_t)(v + ws->res[(Y0 + y) * 16 + X0 + x]));
 			if (on) YT(X0 + x, Y0 + y) = (uint8_t)v;   /* the reads above touch only samples outside the two blocks of this step */
 			__syncwarp();
 		}
@@ -419,8 +451,8 @@ __device__ __noinline__ void intra_luma(WarpSmem *ws, const E264MbRec *r, int la
 			const int X0 = (i & 1) * 8, Y0 = (i >> 1) * 8, x = lane & 7, y = lane >> 3;
 			int v0, v1;
 			pred8x8_warp(ws, X0, Y0, r->modes[i], taps0, taps1, lane, v0, v1);
-			v0 = clip255((short)(v0 + ws->res[(Y0 + y) * 16 + X0 + x]));
-			v1 = clip255((short)(v1 + ws->res[(Y0 + y + 4) * 16 + X0 + x]));
+			v0 = mc_clip255((int16_t)(v0 + ws->res[(Y0 + y) * 16 + X0 + x]));
+			v1 = mc_clip255((int16_t)(v1 + ws->res[(Y0 + y + 4) * 16 + X0 + x]));
 			YT(X0 + x, Y0 + y) = (uint8_t)v0; YT(X0 + x, Y0 + y + 4) = (uint8_t)v1;
 			__syncwarp();
 		}
@@ -447,10 +479,10 @@ __device__ __noinline__ void intra_luma(WarpSmem *ws, const E264MbRec *r, int la
 			const int base = a + c * (y - 7) + 16 + b * (x0 - 7);
 			p0 = p1 = 0;
 #pragma unroll
-			for (int k = 0; k < 4; k++) { p0 |= (uint32_t)clip255((base + b * k) >> 5) << (8 * k); p1 |= (uint32_t)clip255((base + b * (k + 4)) >> 5) << (8 * k); }
+			for (int k = 0; k < 4; k++) { p0 |= (uint32_t)mc_clip255((base + b * k) >> 5) << (8 * k); p1 |= (uint32_t)mc_clip255((base + b * (k + 4)) >> 5) << (8 * k); }
 		}
 		const uint4 rs = *(const uint4 *)&ws->res[y * 16 + x0];
-		*(uint2 *)&YT(x0, y) = make_uint2(intra_add_res4(p0, rs.x, rs.y), intra_add_res4(p1, rs.z, rs.w));   /* the reads above touch only samples outside the macroblock */
+		*(uint2 *)&YT(x0, y) = make_uint2(mc_add_res4(p0, rs.x, rs.y), mc_add_res4(p1, rs.z, rs.w));   /* the reads above touch only samples outside the macroblock */
 		__syncwarp();
 	}
 }
@@ -484,16 +516,35 @@ __device__ __noinline__ void intra_chroma(WarpSmem *ws, const E264MbRec *r, int 
 		const int base = a + c * (y - 3) + 16 + b * (x0 - 3);
 		p = 0;
 #pragma unroll
-		for (int k = 0; k < 4; k++) p |= (uint32_t)clip255((base + b * k) >> 5) << (8 * k);
+		for (int k = 0; k < 4; k++) p |= (uint32_t)mc_clip255((base + b * k) >> 5) << (8 * k);
 	}
 	const uint2 rs = *(const uint2 *)&ws->res[256 + pl * 64 + y * 8 + x0];
-	*(uint32_t *)&CT(pl, x0, y) = intra_add_res4(p, rs.x, rs.y);   /* the reads above touch only the row above / column left of the block */
+	*(uint32_t *)&CT(pl, x0, y) = mc_add_res4(p, rs.x, rs.y);   /* the reads above touch only the row above / column left of the block */
 	__syncwarp();
 }
 
 /* ------------------------------------------------------------------------------------------ */
 /* shared by the reconstruction kernels                                                         */
 /* ------------------------------------------------------------------------------------------ */
+/* sample (0, 0) of macroblock (mbx, mby) in the destination picture: Y in the luma plane, C in the interleaved chroma rows */
+__device__ __forceinline__ void mb_planes(const PicJob &J, int mbx, int mby, uint8_t *&Y, uint8_t *&C) {
+	uint8_t *dst = J.frames + (size_t)J.dst_slot * J.frame_bytes;
+	Y = dst + (size_t)(mby * 16) * J.stride_y + mbx * 16; C = dst + J.plane_y + (size_t)(mby * 8) * J.stride_c + mbx * 8;
+}
+/* the row above the macroblock from the picture into tile row -1 (luma x = -1..23, chroma x = -1..7; x = -1 only with
+ * `left`, luma x >= 16 only with `right`): Ya, Ca point at sample (0, -1) of luma and of Cb, Cr follows cpl bytes further */
+__device__ __forceinline__ void load_row_above(WarpSmem *ws, const uint8_t *Ya, const uint8_t *Ca, int cpl, bool left, bool right, int lane) {
+	const int x = lane - 1;
+	if (x < 24 && (x >= 0 || left) && (x < 16 || right)) YT(x, -1) = __ldcg(Ya + x);
+	if (lane < 18) { const int pl = lane / 9, cx = lane % 9 - 1; if (cx >= 0 || left) CT(pl, cx, -1) = __ldcg(Ca + pl * cpl + cx); }
+}
+/* the raw samples of an I_PCM macroblock (its 384-byte "coefficient run") into the tile */
+__device__ __forceinline__ void load_pcm(WarpSmem *ws, const PicJob &J, const E264MbRec *r, int lane) {
+	const uint8_t *s = (const uint8_t *)(J.coefs + r->coef_off);
+	if (lane < 16) *(uint4 *)&YT(0, lane) = __ldg((const uint4 *)s + lane);
+	else { const int j = lane - 16; *(uint2 *)&CT(j >> 3, 0, j & 7) = __ldg((const uint2 *)(s + 256) + j); }
+	__syncwarp();
+}
 __device__ __forceinline__ void store_mb(WarpSmem *ws, const PicJob &J, uint8_t *Y, uint8_t *C, int lane) {
 	const int cpl = J.stride_c >> 1;
 	if (lane < 16) *(uint4 *)(Y + (size_t)lane * J.stride_y) = *(const uint4 *)&YT(0, lane);
@@ -510,5 +561,9 @@ __device__ __forceinline__ int rec_coef_count(const E264MbRec *r) {
 	if (coded & (CODED_CB_DC | CODED_CR_DC)) n += 8;
 	n += 16 * __popc((coded >> 16) & 0xff);
 	return n;
+}
+/* lane 0 starts the copy of the record's coefficient run into dst (shared memory); it completes on bar */
+__device__ __forceinline__ void coef_request(const PicJob &J, const E264MbRec *r, int16_t *dst, unsigned long long *bar, int lane) {
+	if (lane == 0) tma_bulk_g2s(dst, J.coefs + r->coef_off, (unsigned)rec_coef_count(r) * 2u, bar);
 }
 

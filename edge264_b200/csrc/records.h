@@ -47,6 +47,10 @@
 #define E264B_RECORDS_H
 #include <stdint.h>
 
+/* widest picture the parser accepts, in macroblocks: the device's row-progress words count a row's macroblocks below
+ * PROG_STRIDE (recon_kernels.cuh) */
+#define E264_MAX_WIDTH_MBS 1023
+
 enum { MBK_I4x4 = 0, MBK_I8x8 = 1, MBK_I16x16 = 2, MBK_IPCM = 3, MBK_INTER = 4 };
 
 /* E264MbRec.flags */

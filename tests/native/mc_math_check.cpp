@@ -58,6 +58,19 @@ int main() {
 			}
 		}
 	}
+	// prediction + residual (every reconstruction kernel): per sample the oracle's clip255((int16_t)(p + r)) (port_recon.c),
+	// residuals over the whole int16 range, near zero and at the wrap
+	for (int it = 0; it < 1000000; it++) {
+		const uint32_t p = rnd() ^ rnd() << 8;
+		int16_t r[4];
+		for (int k = 0; k < 4; k++) { const int m = rnd() % 3; r[k] = (int16_t)(m == 0 ? rnd() : m == 1 ? (int)(rnd() % 600) - 300 : 32767 - (int)(rnd() % 300)); }
+		const uint32_t got = mc_add_res4(p, (uint16_t)r[0] | (uint32_t)(uint16_t)r[1] << 16, (uint16_t)r[2] | (uint32_t)(uint16_t)r[3] << 16);
+		for (int k = 0; k < 4; k++) {
+			const int s = (int16_t)(((p >> (8 * k)) & 255) + r[k]), want = s < 0 ? 0 : s > 255 ? 255 : s;
+			n++;
+			if ((int)((got >> (8 * k)) & 255) != want && bad++ < 10) printf("add_res4 mismatch p %08x r %d: want %d got %d\n", p, r[k], want, (int)((got >> (8 * k)) & 255));
+		}
+	}
 	printf("%ld samples checked, %ld mismatches\n", n, bad);
 	return bad != 0;
 }
