@@ -191,7 +191,7 @@ struct Edge264Decoder {
 	Pic pics[E264_MAX_SLOTS];
 	int cur;                           /* slot of the picture being decoded, -1 none */
 	int cur_idr, cur_nal_ref_idc;
-	int prev_ref_frame_num, prev_poc_msb;
+	int prev_ref_frame_num, prev_ref_poc;   /* frame_num and POC of the previous reference picture (8.2.1) */
 	int q_prev_ref_frame_num, q_cur_frame_num;   /* reference-style absolute frame numbers, only used to number FrameIds like it */
 	int32_t next_uid;
 	SliceHeader sh;                    /* header of the slice being parsed */

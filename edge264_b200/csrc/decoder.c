@@ -623,7 +623,7 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	o->frame_crop_offsets[0] = (int16_t)s->crop[2]; o->frame_crop_offsets[1] = (int16_t)s->crop[1];
 	o->frame_crop_offsets[2] = (int16_t)s->crop[3]; o->frame_crop_offsets[3] = (int16_t)s->crop[0];
 	d->configured = 1;
-	if (!keep_numbering) { d->q_prev_ref_frame_num = -1; d->prev_ref_frame_num = -1; d->prev_poc_msb = 0; }
+	if (!keep_numbering) { d->q_prev_ref_frame_num = -1; d->prev_ref_frame_num = -1; d->prev_ref_poc = 0; }
 	return 0;
 }
 
@@ -795,184 +795,202 @@ static int find_free_slot(Edge264Decoder *d) {
 	return pick;
 }
 
-/* Parses the slice header, starts a picture when it is the first slice of one and queues the slice's data on the
- * picture's build.  *jobp is set to NULL once the job is queued; until then it stays the caller's. */
-static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, BitReader *b, SliceJob **jobp) {
-	SliceHeader *h = &d->sh;
-	const PPS *p = NULL;
-	int ret = parse_slice_header(d, b, nal_unit_type, nal_ref_idc, h, &p);
-	if (ret) return ret;
+/* 8.2.1 PicOrderCnt and TopFieldOrderCnt of a frame, from its absolute (unwrapped) frame number */
+static void picture_poc(const Edge264Decoder *d, const SliceHeader *h, int idr, int nal_ref_idc, int frame_num_abs, int *poc, int *poc_top) {
 	const SPS *s = &d->sps;
-	if (!d->configured) return EBADMSG;
-	int idr = nal_unit_type == 5;
-	int mask = (1 << s->log2_max_frame_num) - 1;
+	if (s->poc_type == 0) {
+		int sh = 32 - s->log2_max_poc_lsb;
+		int prev_poc = idr ? 0 : d->prev_ref_poc;
+		int inc = (int)((unsigned)(h->poc_lsb - prev_poc) << sh) >> sh;
+		*poc = *poc_top = prev_poc + inc;
+		if (h->delta_poc_bottom < 0) *poc += h->delta_poc_bottom;   /* PicOrderCnt = min(top, bottom) */
+	} else if (s->poc_type == 1) {
+		int abs_fn = s->num_ref_frames_in_poc_cycle > 0 ? frame_num_abs : 0;
+		if (nal_ref_idc == 0 && abs_fn > 0) abs_fn--;
+		int top = h->delta_poc[0] + (nal_ref_idc ? 0 : s->offset_for_non_ref_pic);
+		if (abs_fn > 0) {
+			int cyc = (abs_fn - 1) / s->num_ref_frames_in_poc_cycle, in = (abs_fn - 1) % s->num_ref_frames_in_poc_cycle, sum = 0, tot = 0;
+			for (int i = 0; i < s->num_ref_frames_in_poc_cycle; i++) { tot += s->offset_for_ref_frame[i]; if (i <= in) sum += s->offset_for_ref_frame[i]; }
+			top += cyc * tot + sum;
+		}
+		int bot = top + s->offset_for_top_to_bottom_field + h->delta_poc[1];
+		*poc = top < bot ? top : bot; *poc_top = top;
+	} else *poc = *poc_top = frame_num_abs * 2 + (nal_ref_idc != 0) - 1;
+}
 
-	/* 7.4.1.2.4 first slice of a new picture? (same tests as the reference, headers.c:1027-1050) */
-	if (d->cur >= 0) {
-		const SliceHeader *f = &d->first_sh;
-		int newpic = h->frame_num != f->frame_num || (nal_ref_idc > 0) != (d->cur_nal_ref_idc > 0) || h->idr_pic_id != f->idr_pic_id ||
-		             (s->poc_type == 0 && h->poc_lsb != f->poc_lsb) || (s->poc_type == 1 && h->delta_poc[0] != f->delta_poc[0]);
-		if (newpic) { ret = finish_picture(d); if (ret) return ret; }
+/* short-term frames the DPB has room for: max_num_ref_frames less the long-term frames */
+static int short_term_room(const Edge264Decoder *d) {
+	int nlong = 0;
+	for (int i = 0; i < d->n_slots; i++) nlong += d->pics[i].in_use && d->pics[i].ref == 2;
+	return d->sps.max_num_ref_frames - nlong;
+}
+
+/* 8.2.5.2 gaps in frame_num (a reference picture was lost): like the reference (headers.c:1095-1139) insert
+ * "non-existing" short-term frames for the missing numbers — they take FrameIds and list positions and push
+ * older pictures out through the sliding window, which keeps the reference indices of the surviving pictures
+ * what the encoder meant.  Their samples are undefined in the reference (never-written buffers); ours are
+ * cleared.  Returns the number of frames inserted. */
+static int fill_frame_num_gap(Edge264Decoder *d, int frame_num_abs) {
+	const SPS *s = &d->sps;
+	int prev = d->prev_ref_frame_num;
+	if (prev < 0 || frame_num_abs - prev <= 1) return 0;
+	int room = short_term_room(d), nshort = 0;
+	for (int i = 0; i < d->n_slots; i++) nshort += d->pics[i].in_use && d->pics[i].ref == 1;
+	int gap_frames = frame_num_abs - prev - 1 < room ? frame_num_abs - prev - 1 : room;
+	if (gap_frames < 0) gap_frames = 0;
+	for (; gap_frames + nshort > room && nshort > 0; nshort--) {
+		int old = -1;
+		for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && d->pics[i].ref == 1 && (old < 0 || d->pics[i].frame_num < d->pics[old].frame_num)) old = i;
+		d->pics[old].ref = 0; slot_release_if_unused(d, old);
 	}
-
-	if (d->cur < 0) {
-		if (d->outq_n > 16) {
-			/* the frame the application is told to fetch may still be with a parser: wait for it here, not in a polling
-			 * loop (without workers every queued frame has been submitted, so this does not wait) */
-			pthread_mutex_lock(&d->lock);
-			while (!__atomic_load_n(&d->hb[d->outq[0]].submitted, __ATOMIC_ACQUIRE)) pthread_cond_wait(&d->done_cv, &d->lock);
-			pthread_mutex_unlock(&d->lock);
-			return ENOBUFS;
+	if (gap_frames > 0) threads_drain(d);   /* the fills below go straight to the device: every earlier picture must be on its way first */
+	for (int fn = frame_num_abs - gap_frames; fn < frame_num_abs; fn++) {
+		int sl = find_free_slot(d);
+		while (sl < 0 && bump_frame(d, -1)) sl = find_free_slot(d);
+		if (sl < 0) { d->next_uid++; continue; }   /* no room even after bumping: keep at least the FrameId numbering */
+		Pic *np = &d->pics[sl];
+		memset(np, 0, sizeof(*np));
+		np->in_use = 1; np->ref = 1; np->nonexisting = 1; np->frame_num = fn; np->uid = d->next_uid++; np->host_buf = -1;
+		int npoc = 0;
+		if (s->poc_type == 2) npoc = fn * 2;
+		else if (s->poc_type == 1 && s->num_ref_frames_in_poc_cycle > 0) {
+			int tot = 0, part = 0, in = fn % s->num_ref_frames_in_poc_cycle;
+			for (int i = 0; i < s->num_ref_frames_in_poc_cycle; i++) { tot += s->offset_for_ref_frame[i]; if (i < in) part += s->offset_for_ref_frame[i]; }
+			npoc = (fn / s->num_ref_frames_in_poc_cycle) * tot + part;   /* as the reference computes it (headers.c:1133-1139), not as 8.2.1 does */
 		}
-		int hbuf = hostbuf_acquire(d);
-		if (hbuf < 0) return ENOBUFS;
-		/* frame_num and POC (8.2.1), with absolute (unwrapped) frame numbers like the reference (headers.c:1059) */
-		int prev = d->prev_ref_frame_num;
-		int frame_num_abs = idr ? 0 : prev + 1 + ((h->frame_num - prev - 1) & mask);
-		if (idr) { d->prev_ref_frame_num = -1; d->prev_poc_msb = 0; }
-		int poc, poc_top;
-		if (s->poc_type == 0) {
-			int sh = 32 - s->log2_max_poc_lsb;
-			int prev_poc = idr ? 0 : d->prev_poc_msb;   /* prev_poc_msb holds the full POC of the previous reference picture */
-			int inc = (int)((unsigned)(h->poc_lsb - prev_poc) << sh) >> sh;
-			poc = poc_top = prev_poc + inc;
-			if (h->delta_poc_bottom < 0) poc += h->delta_poc_bottom;   /* PicOrderCnt = min(top, bottom) */
-		} else if (s->poc_type == 1) {
-			int abs_fn = s->num_ref_frames_in_poc_cycle > 0 ? frame_num_abs : 0;
-			if (nal_ref_idc == 0 && abs_fn > 0) abs_fn--;
-			int top = h->delta_poc[0] + (nal_ref_idc ? 0 : s->offset_for_non_ref_pic);
-			if (abs_fn > 0) {
-				int cyc = (abs_fn - 1) / s->num_ref_frames_in_poc_cycle, in = (abs_fn - 1) % s->num_ref_frames_in_poc_cycle, sum = 0, tot = 0;
-				for (int i = 0; i < s->num_ref_frames_in_poc_cycle; i++) { tot += s->offset_for_ref_frame[i]; if (i <= in) sum += s->offset_for_ref_frame[i]; }
-				top += cyc * tot + sum;
-			}
-			int bot = top + s->offset_for_top_to_bottom_field + h->delta_poc[1];
-			poc = top < bot ? top : bot; poc_top = top;
-		} else poc = poc_top = frame_num_abs * 2 + (nal_ref_idc != 0) - 1;
-
-		/* 8.2.5.2 gaps in frame_num (a reference picture was lost): like the reference (headers.c:1095-1139) insert
-		 * "non-existing" short-term frames for the missing numbers — they take FrameIds and list positions and push
-		 * older pictures out through the sliding window, which keeps the reference indices of the surviving pictures
-		 * what the encoder meant.  Their samples are undefined in the reference (never-written buffers); ours are
-		 * cleared. */
-		int gap_frames = 0;
-		if (!idr && prev >= 0 && frame_num_abs - prev > 1) {
-			int nlong = 0, nshort = 0;
-			for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use) { nlong += d->pics[i].ref == 2; nshort += d->pics[i].ref == 1; }
-			int room = s->max_num_ref_frames - nlong;
-			gap_frames = frame_num_abs - prev - 1 < room ? frame_num_abs - prev - 1 : room;
-			if (gap_frames < 0) gap_frames = 0;
-			for (; gap_frames + nshort > room && nshort > 0; nshort--) {
-				int old = -1;
-				for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && d->pics[i].ref == 1 && (old < 0 || d->pics[i].frame_num < d->pics[old].frame_num)) old = i;
-				d->pics[old].ref = 0; slot_release_if_unused(d, old);
-			}
-			if (gap_frames > 0) threads_drain(d);   /* the fills below go straight to the device: every earlier picture must be on its way first */
-			for (int fn = frame_num_abs - gap_frames; fn < frame_num_abs; fn++) {
-				int sl = find_free_slot(d);
-				while (sl < 0 && bump_frame(d, -1)) sl = find_free_slot(d);
-				if (sl < 0) { d->next_uid++; continue; }   /* no room even after bumping: keep at least the FrameId numbering */
-				Pic *np = &d->pics[sl];
-				memset(np, 0, sizeof(*np));
-				np->in_use = 1; np->ref = 1; np->nonexisting = 1; np->frame_num = fn; np->uid = d->next_uid++; np->host_buf = -1;
-				int npoc = 0;
-				if (s->poc_type == 2) npoc = fn * 2;
-				else if (s->poc_type == 1 && s->num_ref_frames_in_poc_cycle > 0) {
-					int tot = 0, part = 0, in = fn % s->num_ref_frames_in_poc_cycle;
-					for (int i = 0; i < s->num_ref_frames_in_poc_cycle; i++) { tot += s->offset_for_ref_frame[i]; if (i < in) part += s->offset_for_ref_frame[i]; }
-					npoc = (fn / s->num_ref_frames_in_poc_cycle) * tot + part;   /* as the reference computes it (headers.c:1133-1139) */
-				}
-				np->poc = np->poc_dec = np->poc_top = np->poc_top_dec = npoc;
-				for (int i = 0; i < E264_MAX_SLOTS; i++) np->slot_uid[i] = -1;
-				if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, 0); pthread_mutex_unlock(&d->be_lock); }
-			}
-			d->prev_ref_frame_num = frame_num_abs - 1;   /* the last inserted frame is the previous reference frame now (headers.c:1131) */
-		}
-
-		int slot = find_free_slot(d);
-		if (slot < 0) {   /* DPB invariant broken (stream exceeds its own limits): drop the oldest output-pending picture */
-			if (!bump_frame(d, -1)) return EBADMSG;
-			slot = find_free_slot(d);
-			if (slot < 0) return ENOBUFS;
-		}
-		Pic *cp = &d->pics[slot];
-		memset(cp, 0, sizeof(*cp));
-		{   /* FrameId numbering: the reference keeps an absolute FrameNum across IDRs, so an IDR after other
-		     * pictures looks like a frame_num gap and non-existing frames take FrameIds (headers.c:1059,1095-1139) */
-			int q = d->q_prev_ref_frame_num;
-			int qfn = q + 1 + (((idr ? 0 : h->frame_num) - q - 1) & mask);
-			int gap = qfn - q;
-			if (gap > 1 && !gap_frames) {   /* a real gap has just been given its frames (and FrameIds) above */
-				int nlong = 0;
-				for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && d->pics[i].ref == 2) nlong++;
-				int room = s->max_num_ref_frames - nlong;
-				d->next_uid += (gap - 1 < room ? gap - 1 : room) > 0 ? (gap - 1 < room ? gap - 1 : room) : 0;
-			}
-			if (gap > 1) d->q_prev_ref_frame_num = qfn - 1;
-			d->q_cur_frame_num = qfn;
-		}
-		cp->in_use = 1; cp->frame_num = frame_num_abs; cp->poc = cp->poc_dec = poc; cp->poc_top = cp->poc_top_dec = poc_top; cp->uid = d->next_uid++; cp->host_buf = hbuf;
-		d->hb[hbuf].state = 1; d->hb[hbuf].frame_id = cp->uid; d->hb[hbuf].borrowed = 0; d->hb[hbuf].submitted = 0;
-		d->cur = slot; d->cur_idr = idr; d->cur_nal_ref_idc = nal_ref_idc;
-		d->first_sh = *h;
-		for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = d->pics[i].in_use ? d->pics[i].uid : -1;
-		PicBuild *pb = build_acquire(d, slot);     /* may wait for a worker to finish a picture */
-		E264Staging stg; memset(&stg, 0, sizeof(stg));
-		int ar;
-		{ PROF_BEGIN; pthread_mutex_lock(&d->be_lock); ar = d->be->acquire_staging(d->be_ctx, slot, &stg); pthread_mutex_unlock(&d->be_lock); PROF_END(1); }
-		if (ar) {   /* give the build back as if it had never been taken (no later picture exists yet) */
-			pthread_mutex_lock(&d->lock); d->next_seq--; d->slot_users[slot]--; d->slot_build[slot] = NULL; pb->in_use = 0; pthread_mutex_unlock(&d->lock);
-			cp->in_use = 0; d->cur = -1; d->hb[hbuf].state = 0;
-			return ENOMEM;
-		}
-		cp->recs = stg.recs;
-		pb->recs = stg.recs; pb->coefs = stg.coefs; pb->slices = stg.slices; pb->intra_list = stg.intra_list; pb->staging = stg.handle;
-		pb->coef_cap = stg.coef_capacity; pb->n_coefs = 0; pb->n_slices = 0; pb->mbs_done = 0; pb->n_intra = 0; pb->any_deblock = 0;
-		pb->slot = slot; pb->host_buf = hbuf; pb->conceal_ref = -1; pb->slice_counter = 0;
-		{ PROF_BEGIN; memset(pb->mbi, 0, (size_t)d->w_mbs * d->h_mbs * sizeof(MbInfo)); PROF_END(4); }
-		/* records need no clearing: every macroblock of a complete picture rewrites its own (sx_one_mb) */
-		d->pb = pb;
-
-		/* IDR / MMCO5: every earlier picture leaves in output order first (reference headers.c:632, 680) */
-		int has_mmco5 = 0;
-		for (int k = 0; k < h->n_mmco; k++) if (h->mmco[k].op == 5) has_mmco5 = 1;
-		if (idr || has_mmco5) {
-			while (bump_frame(d, slot));
-			if (has_mmco5) { cp->poc_top -= cp->poc; cp->poc = 0; }   /* tempPicOrderCnt subtraction (8.2.1) for output order and later pictures; frame_num restarts in apply_marking, once the picture's own lists and operations have used the real value */
-		}
-		/* C.4.5.3 bumping before insertion (reference headers.c:1229-1250) */
-		int max_bump = s->max_num_ref_frames;
-		if (!nal_ref_idc) {
-			max_bump = 0;
-			for (int i = 0; i < d->n_slots; i++) if (i != slot && d->pics[i].in_use && d->pics[i].needed_for_output && d->pics[i].poc_top < cp->poc_top) max_bump++;
-		}
-		while (dpb_fullness(d) >= s->max_dec_frame_buffering && max_bump--) bump_frame(d, slot);
-		cp->needed_for_output = 1;
-		if (max_bump < 0) {   /* nothing may precede it: straight to the output queue (it is returned once decoded) */
-			cp->needed_for_output = 0;
-			d->hb[hbuf].state = 2; d->outq[d->outq_n++] = hbuf;
-		} else if (waiting_for_output(d) > s->max_num_reorder_frames) bump_frame(d, -1);
-		/* POC bookkeeping for the next picture (8.2.1.1) */
-		if (nal_ref_idc) { d->prev_poc_msb = has_mmco5 ? cp->poc_top : poc_top; }
-		if (has_mmco5) d->prev_ref_frame_num = 0;
+		np->poc = np->poc_dec = np->poc_top = np->poc_top_dec = npoc;
+		for (int i = 0; i < E264_MAX_SLOTS; i++) np->slot_uid[i] = -1;
+		if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, 0); pthread_mutex_unlock(&d->be_lock); }
 	}
+	d->prev_ref_frame_num = frame_num_abs - 1;   /* the last inserted frame is the previous reference frame now (headers.c:1131) */
+	return gap_frames;
+}
 
+/* FrameId numbering: the reference keeps an absolute FrameNum across IDRs, so an IDR after other pictures looks like a
+ * frame_num gap and non-existing frames take FrameIds (headers.c:1059,1095-1139) */
+static void number_frame_id(Edge264Decoder *d, int frame_num, int gap_frames) {
+	int q = d->q_prev_ref_frame_num;
+	int qfn = q + 1 + ((frame_num - q - 1) & ((1 << d->sps.log2_max_frame_num) - 1));
+	int gap = qfn - q;
+	if (gap > 1 && !gap_frames) {   /* a real gap has just been given its frames (and FrameIds) by fill_frame_num_gap */
+		int room = short_term_room(d), n = gap - 1 < room ? gap - 1 : room;
+		if (n > 0) d->next_uid += n;
+	}
+	if (gap > 1) d->q_prev_ref_frame_num = qfn - 1;
+	d->q_cur_frame_num = qfn;
+}
+
+/* first slice of a picture: frame number, POC, FrameId, host buffer, slot, build and staging, bumping; sets d->cur, d->pb */
+static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int nal_ref_idc) {
+	const SPS *s = &d->sps;
+	if (d->outq_n > 16) {
+		/* the frame the application is told to fetch may still be with a parser: wait for it here, not in a polling
+		 * loop (without workers every queued frame has been submitted, so this does not wait) */
+		pthread_mutex_lock(&d->lock);
+		while (!__atomic_load_n(&d->hb[d->outq[0]].submitted, __ATOMIC_ACQUIRE)) pthread_cond_wait(&d->done_cv, &d->lock);
+		pthread_mutex_unlock(&d->lock);
+		return ENOBUFS;
+	}
+	int hbuf = hostbuf_acquire(d);
+	if (hbuf < 0) return ENOBUFS;
+	/* absolute (unwrapped) frame numbers like the reference (headers.c:1059) */
+	int prev = d->prev_ref_frame_num;
+	int frame_num_abs = idr ? 0 : prev + 1 + ((h->frame_num - prev - 1) & ((1 << s->log2_max_frame_num) - 1));
+	if (idr) { d->prev_ref_frame_num = -1; d->prev_ref_poc = 0; }
+	int poc, poc_top;
+	picture_poc(d, h, idr, nal_ref_idc, frame_num_abs, &poc, &poc_top);
+	int gap_frames = idr ? 0 : fill_frame_num_gap(d, frame_num_abs);
+
+	int slot = find_free_slot(d);
+	if (slot < 0) {   /* DPB invariant broken (stream exceeds its own limits): drop the oldest output-pending picture */
+		if (!bump_frame(d, -1)) return EBADMSG;
+		slot = find_free_slot(d);
+		if (slot < 0) return ENOBUFS;
+	}
+	Pic *cp = &d->pics[slot];
+	memset(cp, 0, sizeof(*cp));
+	number_frame_id(d, idr ? 0 : h->frame_num, gap_frames);
+	cp->in_use = 1; cp->frame_num = frame_num_abs; cp->poc = cp->poc_dec = poc; cp->poc_top = cp->poc_top_dec = poc_top; cp->uid = d->next_uid++; cp->host_buf = hbuf;
+	d->hb[hbuf].state = 1; d->hb[hbuf].frame_id = cp->uid; d->hb[hbuf].borrowed = 0; d->hb[hbuf].submitted = 0;
+	d->cur = slot; d->cur_idr = idr; d->cur_nal_ref_idc = nal_ref_idc;
+	d->first_sh = *h;
+	for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = d->pics[i].in_use ? d->pics[i].uid : -1;
+	PicBuild *pb = build_acquire(d, slot);     /* may wait for a worker to finish a picture */
+	E264Staging stg; memset(&stg, 0, sizeof(stg));
+	int ar;
+	{ PROF_BEGIN; pthread_mutex_lock(&d->be_lock); ar = d->be->acquire_staging(d->be_ctx, slot, &stg); pthread_mutex_unlock(&d->be_lock); PROF_END(1); }
+	if (ar) {   /* give the build back as if it had never been taken (no later picture exists yet) */
+		pthread_mutex_lock(&d->lock); d->next_seq--; d->slot_users[slot]--; d->slot_build[slot] = NULL; pb->in_use = 0; pthread_mutex_unlock(&d->lock);
+		cp->in_use = 0; d->cur = -1; d->hb[hbuf].state = 0;
+		return ENOMEM;
+	}
+	cp->recs = stg.recs;
+	pb->recs = stg.recs; pb->coefs = stg.coefs; pb->slices = stg.slices; pb->intra_list = stg.intra_list; pb->staging = stg.handle;
+	pb->coef_cap = stg.coef_capacity; pb->n_coefs = 0; pb->n_slices = 0; pb->mbs_done = 0; pb->n_intra = 0; pb->any_deblock = 0;
+	pb->slot = slot; pb->host_buf = hbuf; pb->conceal_ref = -1; pb->slice_counter = 0;
+	{ PROF_BEGIN; memset(pb->mbi, 0, (size_t)d->w_mbs * d->h_mbs * sizeof(MbInfo)); PROF_END(4); }
+	/* records need no clearing: every macroblock of a complete picture rewrites its own (sx_one_mb) */
+	d->pb = pb;
+
+	/* IDR / MMCO5: every earlier picture leaves in output order first (reference headers.c:632, 680) */
+	int has_mmco5 = 0;
+	for (int k = 0; k < h->n_mmco; k++) if (h->mmco[k].op == 5) has_mmco5 = 1;
+	if (idr || has_mmco5) {
+		while (bump_frame(d, slot));
+		if (has_mmco5) { cp->poc_top -= cp->poc; cp->poc = 0; }   /* tempPicOrderCnt subtraction (8.2.1) for output order and later pictures; frame_num restarts in apply_marking, once the picture's own lists and operations have used the real value */
+	}
+	/* C.4.5.3 bumping before insertion (reference headers.c:1229-1250) */
+	int max_bump = s->max_num_ref_frames;
+	if (!nal_ref_idc) {
+		max_bump = 0;
+		for (int i = 0; i < d->n_slots; i++) if (i != slot && d->pics[i].in_use && d->pics[i].needed_for_output && d->pics[i].poc_top < cp->poc_top) max_bump++;
+	}
+	while (dpb_fullness(d) >= s->max_dec_frame_buffering && max_bump--) bump_frame(d, slot);
+	cp->needed_for_output = 1;
+	if (max_bump < 0) {   /* nothing may precede it: straight to the output queue (it is returned once decoded) */
+		cp->needed_for_output = 0;
+		d->hb[hbuf].state = 2; d->outq[d->outq_n++] = hbuf;
+	} else if (waiting_for_output(d) > s->max_num_reorder_frames) bump_frame(d, -1);
+	/* POC bookkeeping for the next picture (8.2.1.1) */
+	if (nal_ref_idc) { d->prev_ref_poc = has_mmco5 ? cp->poc_top : poc_top; }
+	if (has_mmco5) d->prev_ref_frame_num = 0;
+	return 0;
+}
+
+/* 8.4.2.3.1 implicit weights from POC distances */
+static void implicit_weights(const SliceCtx *c, E264SliceRec *sr) {
+	for (int i0 = 0; i0 < c->num_ref[0] && i0 < 16; i0++) for (int i1 = 0; i1 < c->num_ref[1] && i1 < 16; i1++) {
+		int w1 = 32;
+		if (c->ref_uid[0][i0] >= 0 && c->ref_uid[1][i1] >= 0 && !c->ref_long[0][i0] && !c->ref_long[1][i1]) {
+			int poc0 = c->ref_poc[0][i0], poc1 = c->ref_poc[1][i1];
+			int tb = c->cur_poc - poc0, td = poc1 - poc0;
+			tb = tb < -128 ? -128 : tb > 127 ? 127 : tb; td = td < -128 ? -128 : td > 127 ? 127 : td;
+			if (td != 0) {
+				int tx = (16384 + (td < 0 ? -td : td) / 2) / td;
+				int dsf = (tb * tx + 32) >> 6; dsf = dsf < -1024 ? -1024 : dsf > 1023 ? 1023 : dsf;
+				if ((dsf >> 2) >= -64 && (dsf >> 2) <= 128) w1 = dsf >> 2;
+			}
+		}
+		sr->implicit_w1[i0][i1] = (int16_t)w1;
+	}
+}
+
+/* slice record (deblocking, weights, scaling lists) and parsing context (reference lists, co-located slot in *col_slot) */
+static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, const BitReader *b, SliceJob *job, int *col_slot) {
+	const SPS *s = &d->sps;
 	PicBuild *pb = d->pb;
 	if (pb->n_slices >= E264_MAX_SLICES) return ENOTSUP;
 	Pic *cp = &d->pics[d->cur];
-	int total = d->w_mbs * d->h_mbs;
-	if (h->first_mb >= total) return EBADMSG;
+	if (h->first_mb >= d->w_mbs * d->h_mbs) return EBADMSG;
 
-	/* slice record: deblocking, weights, scaling lists */
 	E264SliceRec *sr = &pb->slices[pb->n_slices];
 	memset(sr, 0, sizeof(*sr));
 	sr->filter_offset_a = (int8_t)h->filter_offset_a; sr->filter_offset_b = (int8_t)h->filter_offset_b;
 	sr->deblock_idc = (uint8_t)h->deblock_idc; sr->slice_type = (uint8_t)h->slice_type;
 	merge_scaling(s, p, sr);
 
-	SliceJob *job = *jobp;
 	SliceCtx *c = &job->sc;
-	int col_slot = -1;
+	*col_slot = -1;
 	c->cabac = p->entropy_coding_mode;
 	c->w_mbs = d->w_mbs; c->h_mbs = d->h_mbs;
 	c->slice_type = h->slice_type; c->slice_id = ++pb->slice_counter; c->slice_idx = pb->n_slices;
@@ -1004,47 +1022,53 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 		}
 		if (h->slice_type == 1 && lists[1][0] >= 0) {
 			c->col_recs = d->pics[lists[1][0]].recs;
-			if (d->pics[lists[1][0]].nonexisting) c->col_recs = NULL; else col_slot = lists[1][0];
+			if (d->pics[lists[1][0]].nonexisting) c->col_recs = NULL; else *col_slot = lists[1][0];
 			/* the co-located picture's Pic entry may be recycled before this slice is parsed: keep a private copy of the uid table */
 			memcpy(job->col_slot_uid, d->pics[lists[1][0]].slot_uid, sizeof(job->col_slot_uid)); c->col_slot_uid = job->col_slot_uid;
 		}
 		int wp = h->slice_type == 0 ? p->weighted_pred_flag : p->weighted_bipred_idc;
 		sr->wp_mode = (uint8_t)wp; sr->luma_log2_wd = (uint8_t)h->luma_log2_wd; sr->chroma_log2_wd = (uint8_t)h->chroma_log2_wd;
 		if (wp == 1) for (int l = 0; l < 2; l++) for (int i = 0; i < 16; i++) for (int k = 0; k < 3; k++) { sr->wp_w[l][i][k] = h->w[l][i][k]; sr->wp_o[l][i][k] = h->o[l][i][k]; }
-		if (wp == 1 && getenv("E264_DEBUG")) for (int l = 0; l <= (h->slice_type == 1); l++) for (int i = 0; i < h->num_ref[l]; i++)
-			fprintf(stderr, "wp l%d ref%d logwd %d/%d w %d %d %d o %d %d %d\n", l, i, h->luma_log2_wd, h->chroma_log2_wd, h->w[l][i][0], h->w[l][i][1], h->w[l][i][2], h->o[l][i][0], h->o[l][i][1], h->o[l][i][2]);
-		if (wp == 2) {   /* 8.4.2.3.1 implicit weights from POC distances */
-			for (int i0 = 0; i0 < h->num_ref[0] && i0 < 16; i0++) for (int i1 = 0; i1 < h->num_ref[1] && i1 < 16; i1++) {
-				int w1 = 32;
-				if (c->ref_uid[0][i0] >= 0 && c->ref_uid[1][i1] >= 0 &&!c->ref_long[0][i0] && !c->ref_long[1][i1]) {
-					int poc0 = c->ref_poc[0][i0], poc1 = c->ref_poc[1][i1];
-					int tb = cp->poc_dec - poc0, td = poc1 - poc0;
-					tb = tb < -128 ? -128 : tb > 127 ? 127 : tb; td = td < -128 ? -128 : td > 127 ? 127 : td;
-					if (td != 0) {
-						int tx = (16384 + (td < 0 ? -td : td) / 2) / td;
-						int dsf = (tb * tx + 32) >> 6; dsf = dsf < -1024 ? -1024 : dsf > 1023 ? 1023 : dsf;
-						if ((dsf >> 2) >= -64 && (dsf >> 2) <= 128) w1 = dsf >> 2;
-					}
-				}
-				sr->implicit_w1[i0][i1] = (int16_t)w1;
-			}
-		}
+		if (wp == 2) implicit_weights(c, sr);
 	}
 	pb->n_slices++;
 	if (h->deblock_idc != 1) pb->any_deblock = 1;
 
-	/* slice data */
 	c->br = *b;
 	c->mbaddr = h->first_mb;
 	c->cabac_init_idc_col = h->slice_type == 2 ? 0 : 1 + h->cabac_init_idc;
-	slice_enqueue(d, pb, job, col_slot);
+	return 0;
+}
+
+/* Parses the slice header, starts a picture when it is the first slice of one and queues the slice's data on the
+ * picture's build.  *jobp is set to NULL once the job is queued; until then it stays the caller's. */
+static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, BitReader *b, SliceJob **jobp) {
+	SliceHeader *h = &d->sh;
+	const PPS *p = NULL;
+	int ret = parse_slice_header(d, b, nal_unit_type, nal_ref_idc, h, &p);
+	if (ret) return ret;
+	const SPS *s = &d->sps;
+	if (!d->configured) return EBADMSG;
+
+	/* 7.4.1.2.4 first slice of a new picture? (same tests as the reference, headers.c:1027-1050) */
+	if (d->cur >= 0) {
+		const SliceHeader *f = &d->first_sh;
+		int newpic = h->frame_num != f->frame_num || (nal_ref_idc > 0) != (d->cur_nal_ref_idc > 0) || h->idr_pic_id != f->idr_pic_id ||
+		             (s->poc_type == 0 && h->poc_lsb != f->poc_lsb) || (s->poc_type == 1 && h->delta_poc[0] != f->delta_poc[0]);
+		if (newpic) { ret = finish_picture(d); if (ret) return ret; }
+	}
+	if (d->cur < 0 && (ret = start_picture(d, h, nal_unit_type == 5, nal_ref_idc))) return ret;
+	int col_slot;
+	if ((ret = setup_slice(d, p, h, b, *jobp, &col_slot))) return ret;
+	PicBuild *pb = d->pb;
+	slice_enqueue(d, pb, *jobp, col_slot);
 	*jobp = NULL;
 	/* With workers, one of them parses the slice data and errors in it are not reported; the picture is closed by the
 	 * next picture's first slice, a flush, the end of the sequence or of the stream.  Without workers, the slice is
 	 * parsed here, its error is returned, and the picture is closed and submitted as soon as it is complete. */
 	if (d->n_threads) return 0;
 	{ PROF_BEGIN; pthread_mutex_lock(&d->lock); ret = build_work(d, pb); pthread_mutex_unlock(&d->lock); PROF_END(0); }
-	if (pb->mbs_done >= total) { int r2 = finish_picture(d); if (!ret) ret = r2; }
+	if (pb->mbs_done >= d->w_mbs * d->h_mbs) { int r2 = finish_picture(d); if (!ret) ret = r2; }
 	return ret;
 }
 
@@ -1085,7 +1109,7 @@ void edge264_flush(Edge264Decoder *d) {
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { d->pics[i].in_use = 0; d->pics[i].host_buf = -1; }
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state != 3 || !d->hb[i].borrowed) d->hb[i].state = 0;
 	d->outq_n = 0; d->cur = -1; d->pending_release = -1;
-	d->prev_ref_frame_num = -1; d->q_prev_ref_frame_num = -1; d->prev_poc_msb = 0;
+	d->prev_ref_frame_num = -1; d->q_prev_ref_frame_num = -1; d->prev_ref_poc = 0;
 	memset(&d->sps, 0, sizeof(d->sps)); memset(d->pps, 0, sizeof(d->pps));
 	d->configured = 0;
 }
