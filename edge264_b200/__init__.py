@@ -59,9 +59,19 @@ def _frame_bytes(f):
     return bytes(out)
 
 
-def decode_bytes(data, lib=None, n_threads=0):
+def _frame_errors(f):
+    """Edge264Frame.mb_errors as bytes (width_mbs x height_mbs of the coded picture, row-major), or None when the decoder
+    reports no macroblock as possibly wrong."""
+    if not f.mb_errors:
+        return None
+    return ctypes.string_at(ctypes.cast(f.mb_errors, ctypes.c_void_p).value, f.stride_mb * (
+        (f.height_Y + f.frame_crop_offsets[0] + f.frame_crop_offsets[2] + 15) >> 4))
+
+
+def decode_bytes(data, lib=None, n_threads=0, errors=False):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
-    Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]."""
+    Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
+    frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -80,7 +90,7 @@ def decode_bytes(data, lib=None, n_threads=0):
         if nal >= end:
             drained = True
         while lib.edge264_get_frame(dec, ctypes.byref(f), 0) == 0:
-            frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)))
+            frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ()))
         if res == errno.ENOBUFS:
             if len(frames) == before:
                 break

@@ -132,6 +132,8 @@ typedef struct SliceCtx {
 	int skip_run, prev_mb_skipped;
 	int n_intra;
 	int error;
+	int missing_ref;          /* a reference-list entry of the slice has no picture (a substitute predicts in its place) */
+	int any_err;              /* a delivered record got a nonzero err (slice_dec.c) */
 	MvCache mc;
 } SliceCtx;
 
@@ -158,6 +160,8 @@ typedef struct PicBuild {
 	uint32_t *intra_list; int staging;
 	int mbs_done, n_intra, any_deblock; uint16_t slice_counter;
 	int slot, host_buf, conceal_ref;
+	int any_err;              /* some record has err != 0 (a slice error, a missing reference, concealment) */
+	uint32_t ref_mask;        /* frame slots the picture's records may predict from */
 	int in_use, closed, running, parsed;
 	uint64_t seq;
 	E264PicDesc pd;           /* filled when parsed: what goes to the backend when the picture's turn comes */
@@ -170,6 +174,8 @@ typedef struct PicBuild {
 typedef struct HostBuf {
 	uint8_t *p;           /* pinned (or user) memory, frame layout of the reference */
 	void *mbs;            /* user mbs allocation when alloc_cb is used (unused by us) */
+	uint8_t *map;         /* pinned host memory: the picture's error map (one byte per macroblock), valid when err_pic */
+	int err_pic;          /* the picture was reconstructed with an error map (E264PicDesc.err_pic) */
 	int state;            /* 0 free, 1 attached to a decoded picture, 2 in the output queue, 3 handed out */
 	int borrowed;
 	int32_t frame_id;
@@ -208,6 +214,7 @@ struct Edge264Decoder {
 	uint64_t next_seq, submit_seq;     /* pictures are submitted to the backend in decoding order */
 	int submitting;                    /* a thread is inside the backend with picture submit_seq */
 	int slot_users[E264_MAX_SLOTS];    /* builds still reading or writing the records of a frame slot */
+	uint32_t taint;                    /* frame slots whose error map may be nonzero (E264PicDesc.taint), in submission order */
 	PicBuild *slot_build[E264_MAX_SLOTS]; uint64_t slot_build_seq[E264_MAX_SLOTS];
 	/* output */
 	HostBuf hb[E264_MAX_HOSTBUFS];
@@ -235,10 +242,16 @@ typedef struct E264Backend {
 	/* reconstruct one picture into `pd->dst_slot` and mirror it into host_out; returns a ticket */
 	int  (*submit)(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint64_t *ticket);
 	int  (*wait)(void *ctx, uint64_t ticket);
-	/* fill a slot with a constant (non-existing frames of frame_num gaps) */
+	/* fill a slot with a constant (non-existing frames of frame_num gaps); its error map becomes all 100 */
 	int  (*fill_slot)(void *ctx, int slot, int y, int c);
 	/* non-blocking form of wait: 0 = the picture is complete, EAGAIN = not yet, < 0 = device error */
 	int  (*poll)(void *ctx, uint64_t ticket);
+	/* error maps (Edge264Frame.mb_errors).  A backend that keeps them has all three; one with NULL here has none, and its
+	 * pictures come out with mb_errors NULL.  submit_maps is submit that also copies the picture's error map into
+	 * host_map when pd->err_pic; pinned_alloc / pinned_free give host memory whatever the output mirrors are. */
+	int  (*submit_maps)(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint64_t *ticket);
+	void *(*pinned_alloc)(void *ctx, size_t bytes);
+	void  (*pinned_free)(void *ctx, void *p);
 } E264Backend;
 const E264Backend *e264_default_backend(void);
 

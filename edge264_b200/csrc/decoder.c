@@ -248,6 +248,16 @@ static int hostbuf_acquire(Edge264Decoder *d) {
 			pthread_mutex_unlock(&d->be_lock);
 			if (!d->hb[i].p) return -1;
 		}
+		/* the error map stays in pinned host memory even when the samples are device memory */
+		if (!d->be->submit_maps) return i;
+		pthread_mutex_lock(&d->be_lock);
+		d->hb[i].map = (uint8_t *)d->be->pinned_alloc(d->be_ctx, (size_t)d->w_mbs * d->h_mbs);
+		pthread_mutex_unlock(&d->be_lock);
+		if (!d->hb[i].map) {
+			if (d->alloc_cb) d->free_cb(d->hb[i].p, d->hb[i].mbs, d->alloc_arg); else d->be->host_free(d->be_ctx, d->hb[i].p);
+			d->hb[i].p = NULL; d->hb[i].mbs = NULL;
+			return -1;
+		}
 		return i;
 	}
 	return -1;
@@ -258,6 +268,7 @@ static void hostbufs_free_all(Edge264Decoder *d) {
 			if (d->alloc_cb) d->free_cb(d->hb[i].p, d->hb[i].mbs, d->alloc_arg);
 			else d->be->host_free(d->be_ctx, d->hb[i].p);
 		}
+		if (d->hb[i].map) d->be->pinned_free(d->be_ctx, d->hb[i].map);
 		memset(&d->hb[i], 0, sizeof(d->hb[i]));
 	}
 	d->outq_n = 0; d->pending_release = -1;
@@ -322,6 +333,7 @@ static void conceal_missing(Edge264Decoder *d, PicBuild *pb) {
 		if (pb->mbi[a].slice_id) continue;
 		E264MbRec *r = pb->recs + a;
 		memset(r, 0, sizeof(*r));
+		r->err = 100;                 /* made up: no slice delivered it */
 		r->qp[0] = r->qp[1] = r->qp[2] = 26;
 		memset(r->ref_idx, -1, sizeof(r->ref_idx)); memset(r->ref_pic, -1, sizeof(r->ref_pic));
 		if (ref >= 0) {
@@ -344,7 +356,11 @@ static int conceal_reference(Edge264Decoder *d) {
  * records are complete afterwards), then hand the picture to the backend (build_submit).  build_work runs both once
  * the picture is closed and every slice of it is parsed. */
 static void build_finalize(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd) {
-	if (pb->mbs_done < d->w_mbs * d->h_mbs) conceal_missing(d, pb);
+	if (pb->mbs_done < d->w_mbs * d->h_mbs) {
+		conceal_missing(d, pb);
+		pb->any_err = 1;
+		if (pb->conceal_ref >= 0) pb->ref_mask |= 1u << pb->conceal_ref;
+	}
 	memset(pd, 0, sizeof(*pd));
 	pd->width_mbs = d->w_mbs; pd->height_mbs = d->h_mbs; pd->stride_y = d->stride_y; pd->stride_c = d->stride_c;
 	pd->plane_y = d->plane_y; pd->frame_bytes = d->frame_bytes; pd->dst_slot = pb->slot;
@@ -354,11 +370,19 @@ static void build_finalize(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd) {
 	for (int a = 0; a < total; a++) if (pb->recs[a].kind != MBK_INTER) pb->intra_list[n++] = (uint32_t)a;
 	pd->n_intra = n;
 }
-static int build_submit(Edge264Decoder *d, PicBuild *pb, const E264PicDesc *pd, uint64_t *ticket) {
+/* called in decoding order: whether the picture needs an error map depends on what the pictures before it left in its
+ * reference slots.  A slot is tainted from the moment a picture with a map (or a non-existing frame) is written into it
+ * until a picture without one is. */
+static int build_submit(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd, uint64_t *ticket) {
 	*ticket = 0;
 	if (pb->host_buf < 0) return 0;
+	pd->err_pic = d->be->submit_maps && (pb->any_err || (pb->ref_mask & d->taint) != 0);
+	pd->taint = d->taint;
+	if (pd->err_pic) d->taint |= 1u << pb->slot; else d->taint &= ~(1u << pb->slot);
+	HostBuf *hb = &d->hb[pb->host_buf];
+	hb->err_pic = pd->err_pic;
 	int r;
-	{ PROF_BEGIN; r = d->be->submit(d->be_ctx, pd, d->hb[pb->host_buf].p, ticket); PROF_END(2); }
+	{ PROF_BEGIN; r = d->be->submit_maps ? d->be->submit_maps(d->be_ctx, pd, hb->p, hb->map, ticket) : d->be->submit(d->be_ctx, pd, hb->p, ticket); PROF_END(2); }
 	return r ? EIO : 0;
 }
 
@@ -452,6 +476,7 @@ static int build_work(Edge264Decoder *d, PicBuild *pb) {
 		int n = e264_parse_slice_data(&job->sc);
 		pb->n_coefs = job->sc.n_coefs; pb->n_intra += job->sc.n_intra;
 		if (n > 0) pb->mbs_done += n;
+		pb->any_err |= job->sc.any_err;
 		if (job->sc.error && !ret) ret = job->sc.error == 2 ? ENOMEM : EBADMSG;
 		free(job->rbsp);
 		pthread_mutex_lock(&d->lock);
@@ -609,6 +634,7 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	}
 	d->pb = NULL;
 	memset(d->slot_users, 0, sizeof(d->slot_users)); memset(d->slot_build, 0, sizeof(d->slot_build));
+	d->taint = 0;
 	pthread_mutex_unlock(&d->lock);
 	if (oom) return ENOMEM;
 	memset(d->pics, 0, sizeof(d->pics));
@@ -861,6 +887,7 @@ static int fill_frame_num_gap(Edge264Decoder *d, int frame_num_abs) {
 		np->poc = np->poc_dec = np->poc_top = np->poc_top_dec = npoc;
 		for (int i = 0; i < E264_MAX_SLOTS; i++) np->slot_uid[i] = -1;
 		if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, 0); pthread_mutex_unlock(&d->be_lock); }
+		d->taint |= 1u << sl;   /* its error map is all 100 */
 	}
 	d->prev_ref_frame_num = frame_num_abs - 1;   /* the last inserted frame is the previous reference frame now (headers.c:1131) */
 	return gap_frames;
@@ -911,7 +938,7 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 	memset(cp, 0, sizeof(*cp));
 	number_frame_id(d, idr ? 0 : h->frame_num, gap_frames);
 	cp->in_use = 1; cp->frame_num = frame_num_abs; cp->poc = cp->poc_dec = poc; cp->poc_top = cp->poc_top_dec = poc_top; cp->uid = d->next_uid++; cp->host_buf = hbuf;
-	d->hb[hbuf].state = 1; d->hb[hbuf].frame_id = cp->uid; d->hb[hbuf].borrowed = 0; d->hb[hbuf].submitted = 0;
+	d->hb[hbuf].state = 1; d->hb[hbuf].frame_id = cp->uid; d->hb[hbuf].borrowed = 0; d->hb[hbuf].submitted = 0; d->hb[hbuf].err_pic = 0;
 	d->cur = slot; d->cur_idr = idr; d->cur_nal_ref_idc = nal_ref_idc;
 	d->first_sh = *h;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = d->pics[i].in_use ? d->pics[i].uid : -1;
@@ -999,7 +1026,7 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 	c->qp = h->slice_qp; c->chroma_qp_offset[0] = p->chroma_qp_index_offset[0]; c->chroma_qp_offset[1] = p->chroma_qp_index_offset[1];
 	c->deblock_idc = h->deblock_idc; c->cur_poc = cp->poc_dec;
 	c->mbi = pb->mbi; c->recs = pb->recs; c->coefs = pb->coefs; c->coef_cap = pb->coef_cap;   /* n_coefs: build_work continues the pool where the previous slice ended */
-	c->col_recs = NULL; c->col_slot_uid = NULL; c->error = 0; c->n_intra = 0;
+	c->col_recs = NULL; c->col_slot_uid = NULL; c->error = 0; c->n_intra = 0; c->missing_ref = 0; c->any_err = 0;
 	memset(c->ref_slot, -1, sizeof(c->ref_slot)); memset(c->ref_long, 0, sizeof(c->ref_long));
 	for (int l = 0; l < 2; l++) for (int i = 0; i < 32; i++) { c->ref_uid[l][i] = -1; c->ref_poc[l][i] = 0; }
 	if (h->slice_type < 2) {
@@ -1016,7 +1043,8 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 			for (int i = 0; i < h->num_ref[l]; i++) {
 				int sl = lists[l][i];
 				c->ref_slot[l][i] = (int8_t)(sl < 0 ? subst : sl);
-				if (sl < 0) continue;
+				pb->ref_mask |= 1u << c->ref_slot[l][i];
+				if (sl < 0) { c->missing_ref = 1; continue; }
 				c->ref_uid[l][i] = d->pics[sl].uid; c->ref_poc[l][i] = d->pics[sl].poc; c->ref_long[l][i] = d->pics[sl].ref == 2;
 			}
 		}
@@ -1209,6 +1237,13 @@ int edge264_get_frame(Edge264Decoder *d, Edge264Frame *out, int borrow) {
 	out->samples[1] = hb->p + d->plane_y + (top >> 1) * d->stride_c + (left >> 1);
 	out->samples[2] = out->samples[1] + (d->stride_c >> 1);
 	out->FrameId = hb->frame_id;
+	/* the map was written for this picture only if some macroblock could be wrong; a map of zeros is reported as none */
+	if (hb->err_pic) {
+		const size_t nmb = (size_t)d->w_mbs * d->h_mbs;
+		size_t k = 0;
+		while (k < nmb && !hb->map[k]) k++;
+		if (k < nmb) { out->mb_errors = hb->map; out->stride_mb = (int16_t)d->w_mbs; }
+	}
 	out->return_arg = (void *)(uintptr_t)(hbuf + 1);
 	hb->state = 3; hb->borrowed = borrow != 0;
 	if (!borrow) d->pending_release = hbuf;   /* valid until the next decode_NAL, as in the reference */

@@ -288,3 +288,21 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 	}
 	PT_FLUSH(16)
 }
+
+/* ---- error map of the inter macroblocks (pictures with err_pic only) ----
+ * A warp per macroblock, lanes over (list, 4x4 block): the largest byte of the reference macroblocks the block's luma
+ * window touches, then the record's own err.  Launched behind e264_inter4_kernel and before the intra kernels, which read
+ * the bytes of inter neighbours.  A kernel of its own: each way of folding this into e264_inter4_kernel (in its step 1, 2
+ * or 3, inlined or as a call) made ptxas spill there, at the 128 registers its 16-warp blocks allow, and clean pictures
+ * would pay for that; here they pay nothing, the launch does not happen. */
+#define MAP_WARPS 8
+__global__ void __launch_bounds__(MAP_WARPS * 32) e264_inter_map_kernel(PicJob J) {
+	const int lane = threadIdx.x & 31, nmb = J.w_mbs * J.h_mbs;
+	uint8_t *dst = map_of(J, J.dst_slot);
+	for (int mb = blockIdx.x * MAP_WARPS + (threadIdx.x >> 5); mb < nmb; mb += gridDim.x * MAP_WARPS) {
+		const E264MbRec *r = J.recs + mb;
+		if (r->kind != MBK_INTER) continue;
+		const unsigned e = __reduce_max_sync(0xffffffffu, map_inter_block(J.maps, J.taint, J.n_slots, J.w_mbs, J.h_mbs, r, lane >> 4, lane & 15, mb % J.w_mbs, mb / J.w_mbs));
+		if (lane == 0) dst[mb] = (uint8_t)max(e, (unsigned)r->err);
+	}
+}

@@ -25,6 +25,7 @@ struct __align__(16) IntraRowsSmem {
 	WarpSmem ws[IR_ROWS][IR_SLOTS];                    /* macroblock x of every row in slot x % IR_SLOTS: residual from the row's transform warp, tile of its prediction warp */
 	uint4 recs[IR_ROWS][IR_RECS][12];           /* records of macroblocks x-4 .. x+3 of every row */
 	uint32_t ring[IR_ROWS][IR_RING][8];         /* bottom sample row of a finished macroblock: luma (4 words), Cb (2), Cr (2) */
+	uint8_t ering[IR_ROWS][IR_RING];            /* and its error map byte (pictures with err_pic) */
 	int16_t coef[IR_ROWS][IR_SLOTS][RES_COEF_MAX];   /* coefficient runs of macroblocks x .. x+3 of every row (cp.async.bulk) */
 	unsigned long long bars[IR_ROWS][IR_SLOTS];
 	uint4 drecs[IR_ROWS][12];                   /* deblocking digests of intra-only pictures: the top neighbour's record */
@@ -110,6 +111,7 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 
 /* The row's PREDICTION warp: waits for the residual, for the row above (top-right neighbour finished) and for room in
  * its ring, predicts into the tile of slot x % IR_SLOTS, stores, hands the bottom sample row down. */
+template <bool MAPS>
 __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &sm, int band, int w, int lane) {
 	const int W = J.w_mbs, H = J.h_mbs;
 	const int lrow = w, mby = band * IR_ROWS + w;
@@ -128,6 +130,7 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 	uint32_t (*ring_out)[8] = sm.ring[lrow];
 	const int cpl = J.stride_c >> 1;
 	int avail = 0;                                            /* macroblocks of the row above the band known to be stored */
+	unsigned eleft = 0;                                       /* lane 0, err_pic: error map byte of the macroblock on the left */
 	PT_DECL
 #pragma unroll 1
 	for (int mbx = 0; mbx < W; mbx++) {
@@ -186,6 +189,23 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 		}
 		__syncwarp();
 		PT_MARK(5)      /* stores */
+		/* ---- error map byte: stored before the publication below that covers the macroblock ---- */
+		if (MAPS && lane == 0) {
+			uint8_t *map = map_of(J, J.dst_slot);
+			unsigned e = r->err;
+			if (kind == MBK_INTER) e = __ldcg(map + mby * W + mbx);      /* written by the inter kernel */
+			else {
+				const unsigned av = map_intra_neighbours(r);
+				auto above = [&](int x) -> unsigned { return from_ring ? sm.ering[lrow - 1][x % IR_RING] : __ldcg(map + (mby - 1) * W + x); };
+				if (av & 1) e = max(e, eleft);
+				if (av & 2) e = max(e, above(mbx));
+				if (av & 4) e = max(e, above(mbx + 1));
+				if (av & 8) e = max(e, above(mbx - 1));
+			}
+			map[mby * W + mbx] = (uint8_t)e;
+			if (to_ring) sm.ering[lrow][mbx % IR_RING] = (uint8_t)e;
+			eleft = e;
+		}
 		/* ---- publish: shared-memory counter for the row below in this band; global counter for the next band, one chunk late ---- */
 		if (lane == 0) {
 			if (to_ring) { __threadfence_block(); *done_out = mbx + 1; }
@@ -211,6 +231,9 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 	}
 }
 
+/* MAPS: the picture has err_pic (recon.cu launches the instantiation that matches it, so clean pictures run code without
+ * any map work) */
+template <bool MAPS>
 __global__ void __launch_bounds__(IR_ROWS * 64) e264_intra_rows_kernel(PicJob J) {
 	TraceScope trace_(J, 2);
 	reset_next_tickets(J);
@@ -230,7 +253,7 @@ __global__ void __launch_bounds__(IR_ROWS * 64) e264_intra_rows_kernel(PicJob J)
 		const int band = sm.band;
 		if (band >= bands) break;
 		if (transform) intra_row_transform(J, sm, band, w, lane, parbits);
-		else intra_row_walk(J, sm, band, w, lane);
+		else intra_row_walk<MAPS>(J, sm, band, w, lane);
 	}
 }
 
@@ -252,6 +275,19 @@ struct __align__(16) IntraTkSmem {
 	int16_t coef[INTRA_WARPS][RES_COEF_MAX];
 	unsigned long long bars[INTRA_WARPS];
 };
+/* The error map byte of an intra macroblock of a P/B picture, once the flags of its neighbours have been seen (lanes 0-3
+ * acquired them, the __syncwarp() behind the waits orders the loads here).  Not inlined: only pictures with err_pic pay. */
+__device__ __noinline__ void intra_error_byte(uint8_t *map, const E264MbRec *r, int mb, int W, int lane) {
+	const unsigned av = map_intra_neighbours(r);
+	int idx = -1;
+	if (lane == 0 && (av & 1)) idx = mb - 1;
+	else if (lane == 1 && (av & 2)) idx = mb - W;
+	else if (lane == 2 && (av & 4)) idx = mb - W + 1;
+	else if (lane == 3 && (av & 8)) idx = mb - W - 1;
+	const unsigned e = __reduce_max_sync(0xffffffffu, idx >= 0 ? (unsigned)__ldcg(map + idx) : 0u);
+	if (lane == 0) map[mb] = (uint8_t)max(e, (unsigned)r->err);
+}
+template <bool MAPS>   /* as for e264_intra_rows_kernel */
 __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) {
 	TraceScope trace_(J, 2);
 	reset_next_tickets(J);
@@ -307,6 +343,7 @@ __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) 
 			store_mb(ws, J, Y, C, lane);
 		}
 		__syncwarp();
+		if (MAPS) intra_error_byte(map_of(J, J.dst_slot), r, mb, W, lane);   /* before the flag: the macroblocks that wait for it read the byte */
 		if (lane == 0) { __threadfence(); *(volatile unsigned *)(J.flags + mb) = J.epoch; }
 		__syncwarp();
 	}

@@ -41,6 +41,7 @@ struct E264bDevice {
 	int dev; cudaStream_t stream;
 	E264PicDesc g; int n_slots; size_t nmb; uint32_t coef_cap;
 	uint8_t *d_frames;
+	uint8_t *d_maps;             /* [n_slots][nmb] error maps of the frame slots (written only for pictures with err_pic) */
 	E264MbRec *h_recs[E264_MAX_SLOTS]; cudaEvent_t rec_up[E264_MAX_SLOTS]; bool rec_busy[E264_MAX_SLOTS];
 	Staging st[NSTAGE]; int stage, n_stage;
 	unsigned *d_sync;            /* synchronisation words, layout SYNC_* in recon_kernels.cuh */
@@ -68,6 +69,8 @@ static void free_geometry(E264bDevice *c) {
 	cudaStreamSynchronize(c->stream);
 	if (c->d_frames) cudaFree(c->d_frames);
 	c->d_frames = NULL;
+	if (c->d_maps) cudaFree(c->d_maps);
+	c->d_maps = NULL;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { if (c->h_recs[i]) cudaFreeHost(c->h_recs[i]); c->h_recs[i] = NULL; c->rec_busy[i] = false; }
 	for (int i = 0; i < NSTAGE; i++) {
 		Staging *s = &c->st[i];
@@ -102,13 +105,15 @@ extern "C" int e264b_create(E264bDevice **out) {
 		}
 	}
 	E264bDevice *c = new E264bDevice();
-	c->dev = 0; c->stream = 0; memset(&c->g, 0, sizeof(c->g)); c->n_slots = 0; c->nmb = 0; c->coef_cap = 0; c->d_frames = NULL;
+	c->dev = 0; c->stream = 0; memset(&c->g, 0, sizeof(c->g)); c->n_slots = 0; c->nmb = 0; c->coef_cap = 0; c->d_frames = NULL; c->d_maps = NULL;
 	memset(c->h_recs, 0, sizeof(c->h_recs)); memset(c->rec_busy, 0, sizeof(c->rec_busy)); memset(c->st, 0, sizeof(c->st)); c->stage = 0; c->d_sync = NULL; c->epoch = 0; c->tick_seq = 0;
 	c->launches = c->h2d_bytes = c->d2h_bytes = 0;
 	c->dev = dev;
-	CK(cudaFuncSetAttribute(e264_intra_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraRowsSmem)));
+	CK(cudaFuncSetAttribute(e264_intra_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraRowsSmem)));
+	CK(cudaFuncSetAttribute(e264_intra_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraRowsSmem)));
 	CK(cudaFuncSetAttribute(e264_inter4_kernel<INTER_MINB0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
-	CK(cudaFuncSetAttribute(e264_intra_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraTkSmem)));
+	CK(cudaFuncSetAttribute(e264_intra_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraTkSmem)));
+	CK(cudaFuncSetAttribute(e264_intra_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraTkSmem)));
 #if INTER_WARPS == 4
 	CK(cudaFuncSetAttribute(e264_inter4_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
 	CK(cudaFuncSetAttribute(e264_inter4_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
@@ -168,6 +173,7 @@ extern "C" int e264b_configure(E264bDevice *c, const E264PicDesc *g, int n_slots
 	size_t pool = (size_t)g->frame_bytes * n_slots;
 	CK(cudaMalloc(&c->d_frames, pool + 256));
 	CK(cudaMemsetAsync(c->d_frames, 128, pool + 256, c->stream));
+	CK(cudaMalloc(&c->d_maps, c->nmb * n_slots));
 	for (int i = 0; i < n_slots; i++) CK(cudaHostAlloc(&c->h_recs[i], c->nmb * sizeof(E264MbRec), cudaHostAllocDefault));
 	for (int i = 0; i < c->n_stage; i++) {
 		Staging *s = &c->st[i];
@@ -212,6 +218,13 @@ extern "C" void e264b_host_free(E264bDevice *c, void *p) {
 	cudaSetDevice(c->dev); free_mirror(p);   /* not ours to pool */
 }
 
+extern "C" void *e264b_pinned_alloc(E264bDevice *c, size_t bytes) {
+	void *p = NULL;
+	cudaSetDevice(c->dev);
+	return cudaHostAlloc(&p, bytes, cudaHostAllocDefault) == cudaSuccess ? p : NULL;
+}
+extern "C" void e264b_pinned_free(E264bDevice *c, void *p) { cudaSetDevice(c->dev); cudaFreeHost(p); }
+
 extern "C" int e264b_acquire_staging(E264bDevice *c, int slot, E264Staging *out) {
 	CK(cudaSetDevice(c->dev));
 	c->stage = (c->stage + 1) % c->n_stage;
@@ -230,6 +243,7 @@ static PicJob make_job(E264bDevice *c, const E264PicDesc *pd, int stage, const E
 	J.err = c->d_sync + SYNC_ERR; J.flags = c->d_sync + SYNC_FLAGS;
 	J.dbk = pd->any_deblock ? c->st[stage].d_dbk : NULL;
 	J.intra_list = intra; J.n_intra = pd->n_intra;
+	J.maps = c->d_maps; J.err_pic = pd->err_pic; J.taint = pd->taint;
 	J.rows_mode = pd->n_intra * 2 > pd->width_mbs * pd->height_mbs;   /* intra pictures: wavefront of row warps */
 	J.trace = NULL; J.trace_base = 0; J.trace_rep = NULL; J.trace_rep_stride = 0; J.diag = 0;
 	if (c->epoch >= PROG_MAX_EPOCH) {   /* restart before the row-progress words leave the range their waits compare in */
@@ -268,17 +282,25 @@ static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd
 #endif
 		e264_inter4_kernel<INTER_MINB0><<<ib, INTER_WARPS * 32, sizeof(InterSmem), c->stream>>>(J);
 		c->launches++;
+		if (J.err_pic) {   /* the error map of the inter macroblocks, before the intra kernels read it */
+			int mb_blocks = (nmb + MAP_WARPS - 1) / MAP_WARPS;
+			e264_inter_map_kernel<<<mb_blocks < cap ? mb_blocks : cap, MAP_WARPS * 32, 0, c->stream>>>(J);
+			c->launches++;
+		}
 	}
 	if (pd->n_intra > 0 && (mask & 2)) {
 		if (J.rows_mode) {   /* intra pictures: bands of rows, hand-over through shared memory */
-			e264_intra_rows_kernel<<<(J.h_mbs + IR_ROWS - 1) / IR_ROWS, IR_ROWS * 64, sizeof(IntraRowsSmem), c->stream>>>(J);
+			const int nb = (J.h_mbs + IR_ROWS - 1) / IR_ROWS;
+			if (J.err_pic) e264_intra_rows_kernel<true><<<nb, IR_ROWS * 64, sizeof(IntraRowsSmem), c->stream>>>(J);
+			else e264_intra_rows_kernel<false><<<nb, IR_ROWS * 64, sizeof(IntraRowsSmem), c->stream>>>(J);
 		} else {
 			/* a warp takes several list entries (E264B_INTRA_DIV, default 2): see INTRA_WARPS */
 			static int idiv = -1;
 			if (idiv < 0) { const char *e = getenv("E264B_INTRA_DIV"); idiv = e && atoi(e) > 0 ? atoi(e) : 2; }
 			int ib = (pd->n_intra + INTRA_WARPS * idiv - 1) / (INTRA_WARPS * idiv);
 			if (ib > cap) ib = cap;
-			e264_intra_kernel<<<ib, INTRA_WARPS * 32, sizeof(IntraTkSmem), c->stream>>>(J);
+			if (J.err_pic) e264_intra_kernel<true><<<ib, INTRA_WARPS * 32, sizeof(IntraTkSmem), c->stream>>>(J);
+			else e264_intra_kernel<false><<<ib, INTRA_WARPS * 32, sizeof(IntraTkSmem), c->stream>>>(J);
 		}
 		c->launches++;
 	}
@@ -293,7 +315,8 @@ static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd
 	return 0;
 }
 
-extern "C" int e264b_submit(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint64_t *ticket) {
+extern "C" int e264b_submit(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint64_t *ticket) { return e264b_submit_maps(c, pd, host_out, NULL, ticket); }
+extern "C" int e264b_submit_maps(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint64_t *ticket) {
 	CK(cudaSetDevice(c->dev));
 	if (pd->staging < 0 || pd->staging >= c->n_stage) return -1;
 	Staging *s = &c->st[pd->staging];
@@ -319,6 +342,7 @@ extern "C" int e264b_submit(E264bDevice *c, const E264PicDesc *pd, uint8_t *host
 	 * be DEVICE memory — unified addressing picks the direction, the frame then reaches the application as device pointers
 	 * without ever crossing PCIe (zero-copy output, SURVEY section 8 f2); E264B_OUTPUT=device makes the decoder's own mirrors device memory */
 	if (host_out) { CK(cudaMemcpyAsync(host_out, c->d_frames + (size_t)pd->dst_slot * pd->frame_bytes, (size_t)pd->frame_bytes - 16, cudaMemcpyDefault, c->stream)); c->d2h_bytes += (size_t)pd->frame_bytes - 16; }
+	if (pd->err_pic && host_map) { CK(cudaMemcpyAsync(host_map, c->d_maps + (size_t)pd->dst_slot * c->nmb, c->nmb, cudaMemcpyDeviceToHost, c->stream)); c->d2h_bytes += c->nmb; }
 	if (c->keep) {
 		KeptPic k; k.pd = *pd;
 		CK(cudaMalloc(&k.d_recs, rec_bytes)); CK(cudaMalloc(&k.d_coefs, coef_bytes + 64)); CK(cudaMalloc(&k.d_slices, sl_bytes + 64)); CK(cudaMalloc(&k.d_intra, in_bytes + 64));
@@ -364,6 +388,14 @@ extern "C" int e264b_fill_slot(E264bDevice *c, int slot, int y, int cc) {
 	uint8_t *f = c->d_frames + (size_t)slot * c->g.frame_bytes;
 	CK(cudaMemsetAsync(f, y, (size_t)c->g.plane_y, c->stream));
 	CK(cudaMemsetAsync(f + c->g.plane_y, cc, (size_t)c->g.frame_bytes - c->g.plane_y, c->stream));
+	CK(cudaMemsetAsync(c->d_maps + (size_t)slot * c->nmb, 100, c->nmb, c->stream));   /* a made-up picture: every macroblock wrong */
+	return 0;
+}
+
+/* the error map of a frame slot as the last picture with err_pic (or fill_slot) left it, into out[nmb] (tests) */
+extern "C" int e264b_slot_map(E264bDevice *c, int slot, uint8_t *out) {
+	CK(cudaSetDevice(c->dev)); CK(cudaStreamSynchronize(c->stream));
+	CK(cudaMemcpy(out, c->d_maps + (size_t)slot * c->nmb, c->nmb, cudaMemcpyDeviceToHost));
 	return 0;
 }
 
@@ -665,9 +697,12 @@ static void *be_host_alloc(void *ctx, size_t b) { return e264b_host_alloc((E264b
 static void be_host_free(void *ctx, void *p) { e264b_host_free((E264bDevice *)ctx, p); }
 static int be_acquire(void *ctx, int slot, E264Staging *out) { return e264b_acquire_staging((E264bDevice *)ctx, slot, out); }
 static int be_submit(void *ctx, const E264PicDesc *pd, uint8_t *out, uint64_t *t) { return e264b_submit((E264bDevice *)ctx, pd, out, t); }
+static int be_submit_maps(void *ctx, const E264PicDesc *pd, uint8_t *out, uint8_t *map, uint64_t *t) { return e264b_submit_maps((E264bDevice *)ctx, pd, out, map, t); }
 static int be_wait(void *ctx, uint64_t t) { return e264b_wait((E264bDevice *)ctx, t); }
 static int be_fill(void *ctx, int slot, int y, int c) { return e264b_fill_slot((E264bDevice *)ctx, slot, y, c); }
 static int be_poll(void *ctx, uint64_t t) { return e264b_poll((E264bDevice *)ctx, t); }
-static const E264Backend cuda_backend = {"cuda-sm_90a", be_create, be_destroy, be_configure, be_host_alloc, be_host_free, be_acquire, be_submit, be_wait, be_fill, be_poll};
+static void *be_pinned_alloc(void *ctx, size_t b) { return e264b_pinned_alloc((E264bDevice *)ctx, b); }
+static void be_pinned_free(void *ctx, void *p) { e264b_pinned_free((E264bDevice *)ctx, p); }
+static const E264Backend cuda_backend = {"cuda-sm_90a", be_create, be_destroy, be_configure, be_host_alloc, be_host_free, be_acquire, be_submit, be_wait, be_fill, be_poll, be_submit_maps, be_pinned_alloc, be_pinned_free};
 extern "C" const E264Backend *e264_default_backend(void) { return &cuda_backend; }
 extern "C" E264bDevice *e264b_of_decoder(Edge264Decoder *d) { return d ? (E264bDevice *)d->be_ctx : NULL; }

@@ -40,6 +40,9 @@ struct PicJob {
 	struct E264DbkMb *dbk;        /* [nmb] deblocking digests written by the inter kernel (the intra-rows kernel in pictures without inter macroblocks); NULL = picture is not deblocked */
 	const uint32_t *intra_list;   /* addresses of the intra macroblocks in raster order */
 	int n_intra;
+	uint8_t *maps;                /* [n_slots][nmb] error maps of the frame slots */
+	int err_pic;                  /* 0: no map is read or written (every map the picture could reach is zeros) */
+	unsigned taint;               /* bit s: slot s's map may be nonzero; a clear bit reads as zeros without a load */
 	unsigned long long *trace;   /* measurement only (e264b_replay): [trace_base + kind] = {first block start, last block end} in globaltimer ns; kinds: 1 inter, 2 intra, 3 deblock */
 	int trace_base;
 	const unsigned *trace_rep;   /* graph replay: device counter of the repetition under way; its slots start trace_rep_stride further on */
@@ -134,6 +137,33 @@ __device__ __forceinline__ int wait_row_progress(const volatile unsigned *p, uns
 }
 /* macroblocks 0 .. n-1 of the row are stored: a gpu-scope fence, then the word */
 __device__ __forceinline__ void publish_row_progress(volatile unsigned *p, unsigned base, int n) { __threadfence(); *p = base + (unsigned)n; }
+/* ---- error maps (PicJob.err_pic): a macroblock's byte is the larger of its record's err and what its prediction reads ---- */
+/* the neighbours an intra macroblock's prediction reads, A=1 B=2 C=4 D=8: A, B, D from the unavailability bits of its
+ * chroma mode, C from the top-right 4x4 block (5) or 8x8 block (1); none for I_PCM, never C for Intra16x16 */
+__device__ __forceinline__ unsigned map_intra_neighbours(const E264MbRec *r) {
+	if (r->kind == MBK_IPCM) return 0;
+	unsigned av = ~(unsigned)(r->chroma_mode >> 4) & 11u;
+	if (r->kind == MBK_I4x4 && !(r->modes[5] & 0x40)) av |= 4;
+	if (r->kind == MBK_I8x8 && !(r->modes[1] & 0x40)) av |= 4;
+	return av;
+}
+/* what 4x4 block z of an inter macroblock inherits through list l: the largest byte of the reference macroblocks its 9x9
+ * luma window (the one mc_load_luma fetches, clamped to the picture: it holds the 6-tap and the chroma footprints) touches,
+ * at most 2x2 of them.  maps = [n_slots][w_mbs * h_mbs]; a slot outside taint reads as zeros. */
+__device__ __forceinline__ unsigned map_inter_block(const uint8_t *maps, unsigned taint, int n_slots, int w_mbs, int h_mbs, const E264MbRec *r, int l, int z, int mbx, int mby) {
+	const int i8 = z >> 2, slot = r->ref_pic[l][i8];
+	if (r->ref_idx[l][i8] < 0 || slot < 0 || slot >= n_slots || !((taint >> slot) & 1u)) return 0;
+	const int W = w_mbs * 16, H = h_mbs * 16;
+	const int X0 = mbx * 16 + blk_x(z) * 4 + (r->mv[l][z][0] >> 2) - 2, Y0 = mby * 16 + blk_y(z) * 4 + (r->mv[l][z][1] >> 2) - 2;
+	const int x0 = min(max(X0, 0), W - 1) >> 4, x1 = min(max(X0 + 8, 0), W - 1) >> 4;
+	const int y0 = min(max(Y0, 0), H - 1) >> 4, y1 = min(max(Y0 + 8, 0), H - 1) >> 4;
+	const uint8_t *m = maps + (size_t)slot * w_mbs * h_mbs;
+	const unsigned a = max(__ldcg(m + y0 * w_mbs + x0), __ldcg(m + y0 * w_mbs + x1));
+	const unsigned b = max(__ldcg(m + y1 * w_mbs + x0), __ldcg(m + y1 * w_mbs + x1));
+	return max(a, b);
+}
+__device__ __forceinline__ uint8_t *map_of(const PicJob &J, int slot) { return J.maps + (size_t)slot * J.w_mbs * J.h_mbs; }
+
 /* ---- shared-memory barrier + TMA helpers (sm_90+ PTX; SASS: SYNCS.*, UBLKCP, UTMALDG) ---- */
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(void *bar, unsigned count) {

@@ -22,7 +22,8 @@
  *
  * The record contract: what the parser guarantees for every picture it submits, damaged input included, and what the
  * kernels rely on (a record outside it may make a kernel read samples nobody wrote, or copy outside the coefficient
- * pool).  oracle/record_check.c checks exactly this list (E264_CHECK_RECORDS=1 on the CPU restatement backend).
+ * pool).  oracle/record_check.c checks this list (E264_CHECK_RECORDS=1 on the CPU restatement backend) but for err, which
+ * the error-map test backend checks.
  *   Picture   dst_slot < n_slots; 1 <= n_slices <= 64; intra_list holds the addresses of the non-inter macroblocks in
  *             raster order and n_intra counts them; any_deblock is set when a macroblock has MBF_DEBLOCK.
  *   Slices    filter_offset_a/b even in -12..12; deblock_idc 0..2; slice_type 0..2; wp_mode 0..2; log2_wd 0..7;
@@ -39,6 +40,7 @@
  *   Deblock   MBF_EDGE_L / MBF_EDGE_T only with MBF_DEBLOCK, never on the picture's left column / top row; MBF_DEBLOCK
  *             only in slices with deblock_idc != 1.  With deblock_idc 0 both edges are set wherever a neighbour exists,
  *             with deblock_idc 2 an edge is set only towards a macroblock of the same slice.
+ *   Error     err <= 100 (checked with the error maps, tests/native/port_maps_backend.c).
  *   Inter     every 8x8 block of an MBK_INTER uses at least one list; a used list has ref_idx 0..15 and a ref_pic in
  *             [0, n_slots) other than dst_slot; an unused list, and every list of an intra macroblock, has -1 in both.
  *             Motion vectors may take any int16 value.
@@ -87,7 +89,8 @@ typedef struct E264MbRec {
 	uint8_t  modes[16];     /* IMODE per luma4x4BlkIdx (Intra4x4) or in [0..3] per 8x8 (Intra8x8) */
 	int8_t   ref_idx[2][4]; /* per list, per 8x8: reference index, -1 = list unused */
 	int8_t   ref_pic[2][4]; /* per list, per 8x8: frame slot of the reference picture, -1 = unused */
-	uint8_t  reserved[16];
+	uint8_t  err;           /* the macroblock's own error, 0..100 (0 = delivered intact; see E264PicDesc.err_pic) */
+	uint8_t  reserved[15];
 	int16_t  mv[2][16][2];  /* per list, per luma4x4BlkIdx: quarter-pel (x, y) */
 } E264MbRec;                /* 192 bytes */
 
@@ -121,6 +124,9 @@ typedef struct E264PicDesc {
 	int32_t any_deblock;          /* at least one macroblock has MBF_DEBLOCK */
 	int32_t n_intra;              /* number of intra macroblocks = entries of the staging's intra_list */
 	int32_t staging;              /* handle of the staging area the picture was written into (E264Staging.handle) */
+	int32_t err_pic;              /* error map wanted: some record has err != 0 or a slot in taint is referenced; with 0 the
+	                               * kernels touch no map and the slot's map counts as all zeros afterwards */
+	uint32_t taint;               /* bit s: frame slot s holds a picture whose map may be nonzero (fill_slot, err_pic) */
 } E264PicDesc;
 
 /* Host-visible staging of one picture, handed out by the backend (pinned memory for the CUDA backend): the parser

@@ -32,10 +32,15 @@ int   e264b_configure(E264bDevice *dev, const struct E264PicDesc *geometry, int 
 void *e264b_host_alloc(E264bDevice *dev, size_t bytes);       /* pinned host memory */
 void  e264b_host_free(E264bDevice *dev, void *p);
 int   e264b_acquire_staging(E264bDevice *dev, int slot, struct E264Staging *out);   /* pinned areas the parser fills; out->handle goes back in E264PicDesc.staging */
+void *e264b_pinned_alloc(E264bDevice *dev, size_t bytes);     /* pinned host memory, whatever E264B_OUTPUT says (error maps) */
+void  e264b_pinned_free(E264bDevice *dev, void *p);
 int   e264b_submit(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, uint64_t *ticket);
+/* e264b_submit that also copies the picture's error map (one byte per macroblock) into host_map when pic->err_pic is set */
+int   e264b_submit_maps(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, uint8_t *host_map, uint64_t *ticket);
 int   e264b_wait(E264bDevice *dev, uint64_t ticket);
 int   e264b_poll(E264bDevice *dev, uint64_t ticket);          /* 0 complete, EAGAIN still on the device, < 0 device error */
-int   e264b_fill_slot(E264bDevice *dev, int slot, int luma, int chroma);
+int   e264b_fill_slot(E264bDevice *dev, int slot, int luma, int chroma);   /* and the slot's error map to all 100 */
+int   e264b_slot_map(E264bDevice *dev, int slot, uint8_t *out);               /* a slot's error map (synchronous) */
 int   e264b_error_flag(E264bDevice *dev);            /* 1 if a dependency wait timed out on the device */
 void  e264b_stats(E264bDevice *dev, uint64_t *kernel_launches, uint64_t *h2d_bytes, uint64_t *d2h_bytes);
 

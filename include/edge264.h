@@ -41,7 +41,9 @@ typedef void (*Edge264FreeCb)(void *samples, void *mbs, void *alloc_arg);
 typedef struct Edge264Frame {
 	const uint8_t *samples[3];      /* Y, Cb, Cr; already offset by the cropping rectangle   */
 	const uint8_t *samples_mvc[3];  /* second view (MVC) — always NULL here                   */
-	const uint8_t *mb_errors;       /* always NULL (as in the reference today)                */
+	const uint8_t *mb_errors;       /* NULL when no macroblock can be wrong, else 0..100 per macroblock of the coded
+	                                 * picture, row y at mb_errors + y * stride_mb (= width in macroblocks); pinned
+	                                 * host memory, valid as long as the samples */
 	int8_t  bit_depth_Y;
 	int8_t  bit_depth_C;
 	int16_t width_Y;
