@@ -21,6 +21,13 @@ class Edge264Frame(ctypes.Structure):
                 ("FrameId_mvc", ctypes.c_int32), ("frame_crop_offsets", ctypes.c_int16 * 4), ("return_arg", ctypes.c_void_p)]
 
 
+class Edge264Motion(ctypes.Structure):
+    """Layout of include/edge264_motion.h: one frame's motion export (pointers into the decoder's buffer of that frame)."""
+    _fields_ = [("mv", ctypes.POINTER(ctypes.c_int16)), ("ref_frame_id", ctypes.POINTER(ctypes.c_int32)),
+                ("mb_type", ctypes.POINTER(ctypes.c_uint8)), ("mb_qp", ctypes.POINTER(ctypes.c_uint8)),
+                ("width_mbs", ctypes.c_int32), ("height_mbs", ctypes.c_int32), ("on_device", ctypes.c_int32)]
+
+
 _loaded = {}
 
 
@@ -45,6 +52,9 @@ def bind(path):
     lib.edge264_decode_NAL.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     lib.edge264_get_frame.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.c_int]
     lib.edge264_return_frame.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+    if hasattr(lib, "edge264_get_motion"):     # the extension of include/edge264_motion.h (absent from the reference's library)
+        lib.edge264_enable_motion.argtypes = [ctypes.c_void_p]
+        lib.edge264_get_motion.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264Motion)]
     _loaded[path] = lib
     return lib
 
@@ -68,10 +78,41 @@ def _frame_errors(f):
         (f.height_Y + f.frame_crop_offsets[0] + f.frame_crop_offsets[2] + 15) >> 4))
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False):
+class _DeviceBytes:
+    """A device buffer as torch sees one (__cuda_array_interface__), to copy it out without another CUDA binding."""
+    def __init__(self, ptr, n):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "strides": None, "version": 3}
+
+
+def frame_motion(lib, dec, f):
+    """The motion export of frame f (just returned by edge264_get_frame) as a dict of numpy arrays (copies):
+    mv int16 [2][4H][4W][2], ref_frame_id int32 [2][2H][2W], mb_type uint8 [H][W], mb_qp uint8 [H][W].  Device memory
+    (on_device) is copied through torch."""
+    import numpy as np
+    m = Edge264Motion()
+    r = lib.edge264_get_motion(dec, ctypes.byref(f), ctypes.byref(m))
+    if r:
+        raise RuntimeError("edge264_get_motion: %s" % errno.errorcode.get(r, r))
+    W, H = m.width_mbs, m.height_mbs
+    out = {}
+    for k, dt, shape in (("mv", np.int16, (2, 4 * H, 4 * W, 2)), ("ref_frame_id", np.int32, (2, 2 * H, 2 * W)),
+                         ("mb_type", np.uint8, (H, W)), ("mb_qp", np.uint8, (H, W))):
+        ptr = ctypes.cast(getattr(m, k), ctypes.c_void_p).value
+        n = int(np.prod(shape)) * np.dtype(dt).itemsize
+        if m.on_device:
+            import torch
+            raw = torch.as_tensor(_DeviceBytes(ptr, n), device="cuda").cpu().numpy()
+        else:
+            raw = np.frombuffer(ctypes.string_at(ptr, n), np.uint8)
+        out[k] = raw.view(dt).reshape(shape)
+    return out
+
+
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
-    frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None."""
+    frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
+    ends with the frame's motion export (frame_motion)."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -80,6 +121,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False):
     dec = lib.edge264_alloc(n_threads, None, None, 0, None, None, None)
     if not dec:
         raise RuntimeError("edge264_alloc failed" + (" (no CUDA device: the GPU backend has no CPU fallback)" if gpu else ""))
+    if motion:
+        r = lib.edge264_enable_motion(dec)
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_enable_motion: %s" % errno.errorcode.get(r, r))
     nal = base + 3 + (1 if data[2] == 0 else 0)
     frames, codes, f = [], [], Edge264Frame()
     drained = False
@@ -90,7 +137,8 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False):
         if nal >= end:
             drained = True
         while lib.edge264_get_frame(dec, ctypes.byref(f), 0) == 0:
-            frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ()))
+            frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ())
+                          + ((frame_motion(lib, dec, f),) if motion else ()))
         if res == errno.ENOBUFS:
             if len(frames) == before:
                 break

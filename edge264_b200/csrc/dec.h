@@ -161,6 +161,7 @@ typedef struct PicBuild {
 	int mbs_done, n_intra, any_deblock; uint16_t slice_counter;
 	int slot, host_buf, conceal_ref;
 	int any_err;              /* some record has err != 0 (a slice error, a missing reference, concealment) */
+	int32_t slot_ids[E264_MAX_SLOTS];   /* FrameId held by every frame slot when the picture started (Pic.slot_uid): the motion export's table */
 	uint32_t ref_mask;        /* frame slots the picture's records may predict from */
 	int in_use, closed, running, parsed;
 	uint64_t seq;
@@ -176,6 +177,9 @@ typedef struct HostBuf {
 	void *mbs;            /* user mbs allocation when alloc_cb is used (unused by us) */
 	uint8_t *map;         /* pinned host memory: the picture's error map (one byte per macroblock), valid when err_pic */
 	int err_pic;          /* the picture was reconstructed with an error map (E264PicDesc.err_pic) */
+	uint8_t *motion;      /* the picture's motion export (records.h E264_MOTION_*), memory of the samples' kind; NULL without export */
+	void *motion_mbs;     /* the mbs allocation alloc_cb returned with it */
+	int motion_dev;       /* motion is device memory */
 	int state;            /* 0 free, 1 attached to a decoded picture, 2 in the output queue, 3 handed out */
 	int borrowed;
 	int32_t frame_id;
@@ -221,6 +225,8 @@ struct Edge264Decoder {
 	int outq[E264_MAX_HOSTBUFS]; int outq_n;
 	int pending_release;               /* host buffer handed out without borrow, released at next decode_NAL */
 	int sync_output;                   /* E264_SYNC_OUTPUT=1: get_frame always waits for the device (the behaviour before round 2's last step; A/B switch) */
+	int motion;                        /* edge264_enable_motion: every output picture carries its motion export */
+	int slices_seen;                   /* a slice NAL unit has been decoded (edge264_enable_motion is refused from then on) */
 	int block_output;                  /* the last decode_NAL asked the application to fetch frames (ENOBUFS, end of stream): get_frame waits for the device */
 	/* scratch: RBSP of the last non-slice NAL unit */
 	uint8_t *rbsp; size_t rbsp_cap;
@@ -252,6 +258,10 @@ typedef struct E264Backend {
 	int  (*submit_maps)(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint64_t *ticket);
 	void *(*pinned_alloc)(void *ctx, size_t bytes);
 	void  (*pinned_free)(void *ctx, void *p);
+	/* motion export (include/edge264_motion.h); NULL: the backend has none.  submit_maps that also writes the picture's
+	 * export into `motion` (E264_MOTION_BYTES per macroblock), with slot_ids[s] the FrameId of frame slot s
+	 * (E264_MAX_SLOTS entries, -1 for an empty slot); *on_device tells whether `motion` is device memory. */
+	int  (*submit_motion)(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint8_t *motion, const int32_t *slot_ids, int *on_device, uint64_t *ticket);
 } E264Backend;
 const E264Backend *e264_default_backend(void);
 

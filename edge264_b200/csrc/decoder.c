@@ -15,6 +15,7 @@
 #include <unistd.h>
 #include "dec.h"
 #include "h264_tables.h"
+#include "../../include/edge264_motion.h"
 
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
@@ -232,45 +233,63 @@ static void merge_scaling(const SPS *s, const PPS *p, E264SliceRec *sr) {
 /* ------------------------------------------------------------------------------------------ */
 /* host mirrors and output queue                                                                */
 /* ------------------------------------------------------------------------------------------ */
+static void hostbuf_free(Edge264Decoder *d, HostBuf *hb) {
+	if (hb->p) {
+		if (d->alloc_cb) d->free_cb(hb->p, hb->mbs, d->alloc_arg);
+		else d->be->host_free(d->be_ctx, hb->p);
+	}
+	if (hb->map) d->be->pinned_free(d->be_ctx, hb->map);
+	if (hb->motion) {
+		if (d->alloc_cb) d->free_cb(hb->motion, hb->motion_mbs, d->alloc_arg);
+		else d->be->host_free(d->be_ctx, hb->motion);
+	}
+	memset(hb, 0, sizeof(*hb));
+}
 static int hostbuf_acquire(Edge264Decoder *d) {
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state == 0 && d->hb[i].p) return i;
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state == 0) {
+		HostBuf *hb = &d->hb[i];
 		size_t bytes = (size_t)d->frame_bytes + 64;
 		if (d->alloc_cb) {
 			void *smp = NULL, *mbs = NULL;
 			/* reference sizes (headers.c:113-117): samples = plane_Y + plane_C + 16, mbs = 304 * ((W+1)*H - 1) */
 			d->alloc_cb(&smp, (unsigned)(d->plane_y + d->plane_c + 16), &mbs, (unsigned)(304 * ((d->w_mbs + 1) * d->h_mbs - 1)), ENOMEM, d->alloc_arg);
 			if (!smp) return -1;
-			d->hb[i].p = (uint8_t *)smp; d->hb[i].mbs = mbs;
+			hb->p = (uint8_t *)smp; hb->mbs = mbs;
 		} else {
 			pthread_mutex_lock(&d->be_lock);
-			d->hb[i].p = (uint8_t *)d->be->host_alloc(d->be_ctx, bytes);
+			hb->p = (uint8_t *)d->be->host_alloc(d->be_ctx, bytes);
 			pthread_mutex_unlock(&d->be_lock);
-			if (!d->hb[i].p) return -1;
+			if (!hb->p) return -1;
 		}
 		/* the error map stays in pinned host memory even when the samples are device memory */
-		if (!d->be->submit_maps) return i;
-		pthread_mutex_lock(&d->be_lock);
-		d->hb[i].map = (uint8_t *)d->be->pinned_alloc(d->be_ctx, (size_t)d->w_mbs * d->h_mbs);
-		pthread_mutex_unlock(&d->be_lock);
-		if (!d->hb[i].map) {
-			if (d->alloc_cb) d->free_cb(d->hb[i].p, d->hb[i].mbs, d->alloc_arg); else d->be->host_free(d->be_ctx, d->hb[i].p);
-			d->hb[i].p = NULL; d->hb[i].mbs = NULL;
-			return -1;
+		if (d->be->submit_maps) {
+			pthread_mutex_lock(&d->be_lock);
+			hb->map = (uint8_t *)d->be->pinned_alloc(d->be_ctx, (size_t)d->w_mbs * d->h_mbs);
+			pthread_mutex_unlock(&d->be_lock);
+			if (!hb->map) { hostbuf_free(d, hb); return -1; }
+		}
+		/* the motion export lives where the samples live: from the application's allocator, else from the backend's
+		 * output mirrors (pinned host memory, device memory with E264B_OUTPUT=device) */
+		if (d->motion) {
+			const size_t mbytes = (size_t)d->w_mbs * d->h_mbs * E264_MOTION_BYTES;
+			if (d->alloc_cb) {
+				void *m = NULL, *mbs = NULL;
+				d->alloc_cb(&m, (unsigned)mbytes, &mbs, 0, ENOMEM, d->alloc_arg);
+				hb->motion = (uint8_t *)m; hb->motion_mbs = mbs;
+			} else {
+				pthread_mutex_lock(&d->be_lock);
+				hb->motion = (uint8_t *)d->be->host_alloc(d->be_ctx, mbytes);
+				pthread_mutex_unlock(&d->be_lock);
+			}
+			if (!hb->motion) { hostbuf_free(d, hb); return -1; }
 		}
 		return i;
 	}
 	return -1;
 }
 static void hostbufs_free_all(Edge264Decoder *d) {
-	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) {
-		if (d->hb[i].p) {
-			if (d->alloc_cb) d->free_cb(d->hb[i].p, d->hb[i].mbs, d->alloc_arg);
-			else d->be->host_free(d->be_ctx, d->hb[i].p);
-		}
-		if (d->hb[i].map) d->be->pinned_free(d->be_ctx, d->hb[i].map);
-		memset(&d->hb[i], 0, sizeof(d->hb[i]));
-	}
+	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) hostbuf_free(d, &d->hb[i]);
 	d->outq_n = 0; d->pending_release = -1;
 }
 
@@ -382,7 +401,12 @@ static int build_submit(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd, uint64
 	HostBuf *hb = &d->hb[pb->host_buf];
 	hb->err_pic = pd->err_pic;
 	int r;
-	{ PROF_BEGIN; r = d->be->submit_maps ? d->be->submit_maps(d->be_ctx, pd, hb->p, hb->map, ticket) : d->be->submit(d->be_ctx, pd, hb->p, ticket); PROF_END(2); }
+	{
+		PROF_BEGIN;
+		if (d->motion) r = d->be->submit_motion(d->be_ctx, pd, hb->p, hb->map, hb->motion, pb->slot_ids, &hb->motion_dev, ticket);
+		else r = d->be->submit_maps ? d->be->submit_maps(d->be_ctx, pd, hb->p, hb->map, ticket) : d->be->submit(d->be_ctx, pd, hb->p, ticket);
+		PROF_END(2);
+	}
 	return r ? EIO : 0;
 }
 
@@ -955,6 +979,7 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 	pb->recs = stg.recs; pb->coefs = stg.coefs; pb->slices = stg.slices; pb->intra_list = stg.intra_list; pb->staging = stg.handle;
 	pb->coef_cap = stg.coef_capacity; pb->n_coefs = 0; pb->n_slices = 0; pb->mbs_done = 0; pb->n_intra = 0; pb->any_deblock = 0;
 	pb->slot = slot; pb->host_buf = hbuf; pb->conceal_ref = -1; pb->slice_counter = 0;
+	memcpy(pb->slot_ids, cp->slot_uid, sizeof(pb->slot_ids));   /* slots may hold other pictures by the time this one is submitted */
 	{ PROF_BEGIN; memset(pb->mbi, 0, (size_t)d->w_mbs * d->h_mbs * sizeof(MbInfo)); PROF_END(4); }
 	/* records need no clearing: every macroblock of a complete picture rewrites its own (sx_one_mb) */
 	d->pb = pb;
@@ -1173,6 +1198,7 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 	int nal_ref_idc = buf[0] >> 5, nal_unit_type = buf[0] & 31;
 	size_t n = (size_t)(end - buf) - 1;
 	if (nal_unit_type == 1 || nal_unit_type == 5) {   /* the slice data is parsed from its own copy of the payload, possibly later */
+		d->slices_seen = 1;
 		SliceJob *job = (SliceJob *)calloc(1, sizeof(SliceJob));
 		/* slack: the slice parsers test for an overrun once per macroblock, so a damaged slice reads past its end */
 		uint8_t *rb = job ? (uint8_t *)malloc(n + 4096) : NULL;
@@ -1254,4 +1280,31 @@ void edge264_return_frame(Edge264Decoder *d, void *return_arg) {
 	if (!d) return;
 	int i = (int)(uintptr_t)return_arg - 1;
 	if (i >= 0 && i < E264_MAX_HOSTBUFS && d->hb[i].state == 3) { d->hb[i].state = 0; d->hb[i].borrowed = 0; if (d->pending_release == i) d->pending_release = -1; }
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* motion export (include/edge264_motion.h)                                                     */
+/* ------------------------------------------------------------------------------------------ */
+int edge264_enable_motion(Edge264Decoder *d) {
+	if (!d) return EINVAL;
+	if (!d->be->submit_motion) return ENOTSUP;
+	if (d->slices_seen) return EBUSY;   /* host buffers are created with the first picture: they would lack the export */
+	d->motion = 1;
+	return 0;
+}
+
+int edge264_get_motion(Edge264Decoder *d, const Edge264Frame *frame, Edge264Motion *out) {
+	if (!d || !frame || !out) return EINVAL;
+	if (!d->motion) return ENOENT;
+	const int i = (int)(uintptr_t)frame->return_arg - 1;
+	if (i < 0 || i >= E264_MAX_HOSTBUFS || d->hb[i].state != 3 || !d->hb[i].motion) return EINVAL;
+	const size_t nmb = (size_t)d->w_mbs * d->h_mbs;
+	const uint8_t *m = d->hb[i].motion;
+	out->mv = (const int16_t *)(m + E264_MOTION_MV * nmb);
+	out->ref_frame_id = (const int32_t *)(m + E264_MOTION_REF * nmb);
+	out->mb_type = m + E264_MOTION_TYPE * nmb;
+	out->mb_qp = m + E264_MOTION_QP * nmb;
+	out->width_mbs = d->w_mbs; out->height_mbs = d->h_mbs;
+	out->on_device = d->hb[i].motion_dev;
+	return 0;
 }

@@ -20,6 +20,7 @@
 #include "deblock_kernels.cuh"
 #include "inter_kernels.cuh"
 #include "intra_kernels.cuh"
+#include "motion_kernels.cuh"
 extern "C" {
 #include "dec.h"
 }
@@ -42,6 +43,7 @@ struct E264bDevice {
 	E264PicDesc g; int n_slots; size_t nmb; uint32_t coef_cap;
 	uint8_t *d_frames;
 	uint8_t *d_maps;             /* [n_slots][nmb] error maps of the frame slots (written only for pictures with err_pic) */
+	uint8_t *d_motion;           /* [nmb * E264_MOTION_BYTES] motion export of the picture last submitted with one (allocated at the first) */
 	E264MbRec *h_recs[E264_MAX_SLOTS]; cudaEvent_t rec_up[E264_MAX_SLOTS]; bool rec_busy[E264_MAX_SLOTS];
 	Staging st[NSTAGE]; int stage, n_stage;
 	unsigned *d_sync;            /* synchronisation words, layout SYNC_* in recon_kernels.cuh */
@@ -71,6 +73,8 @@ static void free_geometry(E264bDevice *c) {
 	c->d_frames = NULL;
 	if (c->d_maps) cudaFree(c->d_maps);
 	c->d_maps = NULL;
+	if (c->d_motion) cudaFree(c->d_motion);
+	c->d_motion = NULL;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { if (c->h_recs[i]) cudaFreeHost(c->h_recs[i]); c->h_recs[i] = NULL; c->rec_busy[i] = false; }
 	for (int i = 0; i < NSTAGE; i++) {
 		Staging *s = &c->st[i];
@@ -105,7 +109,7 @@ extern "C" int e264b_create(E264bDevice **out) {
 		}
 	}
 	E264bDevice *c = new E264bDevice();
-	c->dev = 0; c->stream = 0; memset(&c->g, 0, sizeof(c->g)); c->n_slots = 0; c->nmb = 0; c->coef_cap = 0; c->d_frames = NULL; c->d_maps = NULL;
+	c->dev = 0; c->stream = 0; memset(&c->g, 0, sizeof(c->g)); c->n_slots = 0; c->nmb = 0; c->coef_cap = 0; c->d_frames = NULL; c->d_maps = NULL; c->d_motion = NULL;
 	memset(c->h_recs, 0, sizeof(c->h_recs)); memset(c->rec_busy, 0, sizeof(c->rec_busy)); memset(c->st, 0, sizeof(c->st)); c->stage = 0; c->d_sync = NULL; c->epoch = 0; c->tick_seq = 0;
 	c->launches = c->h2d_bytes = c->d2h_bytes = 0;
 	c->dev = dev;
@@ -317,7 +321,11 @@ static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd
 
 extern "C" int e264b_submit(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint64_t *ticket) { return e264b_submit_maps(c, pd, host_out, NULL, ticket); }
 extern "C" int e264b_submit_maps(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint64_t *ticket) {
+	return e264b_submit_motion(c, pd, host_out, host_map, NULL, NULL, 0, NULL, ticket);
+}
+extern "C" int e264b_submit_motion(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint8_t *motion, const int32_t *slot_ids, int n_ids, int *on_device, uint64_t *ticket) {
 	CK(cudaSetDevice(c->dev));
+	if (motion && (n_ids < 0 || n_ids > MOTION_MAX_SLOTS)) return -1;
 	if (pd->staging < 0 || pd->staging >= c->n_stage) return -1;
 	Staging *s = &c->st[pd->staging];
 	size_t rec_bytes = c->nmb * sizeof(E264MbRec), coef_bytes = ((size_t)pd->n_coefs * 2 + 15) & ~(size_t)15, sl_bytes = (size_t)pd->n_slices * sizeof(E264SliceRec);
@@ -343,6 +351,18 @@ extern "C" int e264b_submit_maps(E264bDevice *c, const E264PicDesc *pd, uint8_t 
 	 * without ever crossing PCIe (zero-copy output, SURVEY section 8 f2); E264B_OUTPUT=device makes the decoder's own mirrors device memory */
 	if (host_out) { CK(cudaMemcpyAsync(host_out, c->d_frames + (size_t)pd->dst_slot * pd->frame_bytes, (size_t)pd->frame_bytes - 16, cudaMemcpyDefault, c->stream)); c->d2h_bytes += (size_t)pd->frame_bytes - 16; }
 	if (pd->err_pic && host_map) { CK(cudaMemcpyAsync(host_map, c->d_maps + (size_t)pd->dst_slot * c->nmb, c->nmb, cudaMemcpyDeviceToHost, c->stream)); c->d2h_bytes += c->nmb; }
+	if (motion) {   /* the motion export, from the records the kernels above read (the staging is not reused before s->done), copied like the samples */
+		const size_t bytes = c->nmb * E264_MOTION_BYTES;
+		if (!c->d_motion) CK(cudaMalloc(&c->d_motion, bytes));
+		MotionIds ids;
+		for (int k = 0; k < MOTION_MAX_SLOTS; k++) ids.id[k] = k < n_ids ? slot_ids[k] : -1;
+		const int runs = (pd->width_mbs + MOTION_RUN - 1) / MOTION_RUN;
+		e264_motion_kernel<<<runs * pd->height_mbs, MOTION_THREADS, 0, c->stream>>>(s->d_recs, pd->width_mbs, pd->height_mbs, ids, c->d_motion);
+		c->launches++;
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(motion, c->d_motion, bytes, cudaMemcpyDefault, c->stream)); c->d2h_bytes += bytes;
+		if (on_device) { cudaPointerAttributes a; *on_device = cudaPointerGetAttributes(&a, motion) == cudaSuccess && a.type == cudaMemoryTypeDevice; cudaGetLastError(); }
+	}
 	if (c->keep) {
 		KeptPic k; k.pd = *pd;
 		CK(cudaMalloc(&k.d_recs, rec_bytes)); CK(cudaMalloc(&k.d_coefs, coef_bytes + 64)); CK(cudaMalloc(&k.d_slices, sl_bytes + 64)); CK(cudaMalloc(&k.d_intra, in_bytes + 64));
@@ -703,6 +723,11 @@ static int be_fill(void *ctx, int slot, int y, int c) { return e264b_fill_slot((
 static int be_poll(void *ctx, uint64_t t) { return e264b_poll((E264bDevice *)ctx, t); }
 static void *be_pinned_alloc(void *ctx, size_t b) { return e264b_pinned_alloc((E264bDevice *)ctx, b); }
 static void be_pinned_free(void *ctx, void *p) { e264b_pinned_free((E264bDevice *)ctx, p); }
-static const E264Backend cuda_backend = {"cuda-sm_90a", be_create, be_destroy, be_configure, be_host_alloc, be_host_free, be_acquire, be_submit, be_wait, be_fill, be_poll, be_submit_maps, be_pinned_alloc, be_pinned_free};
+static int be_submit_motion(void *ctx, const E264PicDesc *pd, uint8_t *out, uint8_t *map, uint8_t *motion, const int32_t *ids, int *on_device, uint64_t *t) {
+	return e264b_submit_motion((E264bDevice *)ctx, pd, out, map, motion, ids, E264_MAX_SLOTS, on_device, t);
+}
+static_assert(E264_MAX_SLOTS <= MOTION_MAX_SLOTS, "the motion kernel's FrameId table holds every frame slot");
+static const E264Backend cuda_backend = {"cuda-sm_90a", be_create, be_destroy, be_configure, be_host_alloc, be_host_free, be_acquire, be_submit, be_wait, be_fill, be_poll, be_submit_maps, be_pinned_alloc, be_pinned_free,
+                                         be_submit_motion};
 extern "C" const E264Backend *e264_default_backend(void) { return &cuda_backend; }
 extern "C" E264bDevice *e264b_of_decoder(Edge264Decoder *d) { return d ? (E264bDevice *)d->be_ctx : NULL; }

@@ -5,6 +5,7 @@
  *   intra_kernels.cuh    e264_intra_kernel       intra macroblocks of P/B pictures, in dependency order (flags)
  *                        e264_intra_rows_kernel  intra pictures: band wavefront
  *   deblock_kernels.cuh  e264_deblock_kernel     boundary strengths + the in-loop filter: band wavefront
+ *   motion_kernels.cuh   e264_motion_kernel      the motion export (decoders that asked for it): records -> raster arrays
  * Up to three launches per picture.  Arithmetic is restated from ITU-T H.264 with the reference's observable integer
  * widths; results are bit-exact with the reference decoder (tests/test_gpu_parity.py). */
 #pragma once

@@ -129,6 +129,14 @@ typedef struct E264PicDesc {
 	uint32_t taint;               /* bit s: frame slot s holds a picture whose map may be nonzero (fill_slot, err_pic) */
 } E264PicDesc;
 
+/* The motion export of one picture (include/edge264_motion.h): one buffer of E264_MOTION_BYTES bytes per macroblock, the
+ * four arrays at these offsets, in bytes per macroblock of the picture (nmb = width_mbs * height_mbs):
+ *   mv            E264_MOTION_MV * nmb    int16 [2][4 height_mbs][4 width_mbs][2]
+ *   ref_frame_id  E264_MOTION_REF * nmb   int32 [2][2 height_mbs][2 width_mbs]
+ *   mb_type       E264_MOTION_TYPE * nmb  uint8 [height_mbs][width_mbs]
+ *   mb_qp         E264_MOTION_QP * nmb    uint8 [height_mbs][width_mbs] */
+enum { E264_MOTION_MV = 0, E264_MOTION_REF = 128, E264_MOTION_TYPE = 160, E264_MOTION_QP = 161, E264_MOTION_BYTES = 162 };
+
 /* Host-visible staging of one picture, handed out by the backend (pinned memory for the CUDA backend): the parser
  * writes records, levels and slice records straight into it; intra_list receives the addresses of the picture's intra
  * macroblocks in raster order (the device schedules them from it). */

@@ -37,6 +37,12 @@ void  e264b_pinned_free(E264bDevice *dev, void *p);
 int   e264b_submit(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, uint64_t *ticket);
 /* e264b_submit that also copies the picture's error map (one byte per macroblock) into host_map when pic->err_pic is set */
 int   e264b_submit_maps(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, uint8_t *host_map, uint64_t *ticket);
+/* e264b_submit_maps that also writes the picture's motion export (include/edge264_motion.h; layout E264_MOTION_* of
+ * edge264_b200/csrc/records.h, 162 bytes per macroblock) into `motion`, host or device memory: slot_ids[s] is the FrameId
+ * of frame slot s for s < n_ids (at most 32), -1 elsewhere; *on_device (if not NULL) tells whether `motion` is device
+ * memory.  With motion NULL it is e264b_submit_maps: no launch, no copy. */
+int   e264b_submit_motion(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, uint8_t *host_map, uint8_t *motion,
+                          const int32_t *slot_ids, int n_ids, int *on_device, uint64_t *ticket);
 int   e264b_wait(E264bDevice *dev, uint64_t ticket);
 int   e264b_poll(E264bDevice *dev, uint64_t ticket);          /* 0 complete, EAGAIN still on the device, < 0 device error */
 int   e264b_fill_slot(E264bDevice *dev, int slot, int luma, int chroma);   /* and the slot's error map to all 100 */
