@@ -28,6 +28,18 @@ class Edge264Motion(ctypes.Structure):
                 ("width_mbs", ctypes.c_int32), ("height_mbs", ctypes.c_int32), ("on_device", ctypes.c_int32)]
 
 
+PACKED_I420, PACKED_NV12 = 0, 1
+
+
+class Edge264Packed(ctypes.Structure):
+    """Layout of include/edge264_packed.h: one frame's packed output (pointers into the decoder's buffer of that frame).
+    Sizes are ceil(cropped size >> log2_scale), strides the row bytes rounded up to 64, planes 256-byte aligned
+    (e264_packed_layout in csrc/records.h)."""
+    _fields_ = [("planes", ctypes.c_void_p * 3), ("stride", ctypes.c_int32 * 3), ("width", ctypes.c_int32), ("height", ctypes.c_int32),
+                ("width_C", ctypes.c_int32), ("height_C", ctypes.c_int32), ("format", ctypes.c_int32), ("log2_scale", ctypes.c_int32),
+                ("on_device", ctypes.c_int32)]
+
+
 _loaded = {}
 
 
@@ -55,6 +67,9 @@ def bind(path):
     if hasattr(lib, "edge264_get_motion"):     # the extension of include/edge264_motion.h (absent from the reference's library)
         lib.edge264_enable_motion.argtypes = [ctypes.c_void_p]
         lib.edge264_get_motion.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264Motion)]
+    if hasattr(lib, "edge264_get_packed"):     # the extension of include/edge264_packed.h
+        lib.edge264_enable_packed.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
+        lib.edge264_get_packed.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264Packed)]
     _loaded[path] = lib
     return lib
 
@@ -108,11 +123,37 @@ def frame_motion(lib, dec, f):
     return out
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False):
+def frame_packed(lib, dec, f):
+    """The packed output of frame f (just returned by edge264_get_frame) as a dict of numpy arrays (copies, strides
+    removed): format, log2_scale, on_device, y [height][width] and cb, cr [height_C][width_C] (I420) or cbcr
+    [height_C][width_C][2] (NV12).  Device memory (on_device) is copied through torch."""
+    import numpy as np
+    p = Edge264Packed()
+    r = lib.edge264_get_packed(dec, ctypes.byref(f), ctypes.byref(p))
+    if r:
+        raise RuntimeError("edge264_get_packed: %s" % errno.errorcode.get(r, r))
+    def plane(i, rows, row_bytes):
+        n = p.stride[i] * (rows - 1) + row_bytes
+        if p.on_device:
+            import torch
+            raw = torch.as_tensor(_DeviceBytes(p.planes[i], n), device="cuda").cpu().numpy()
+        else:
+            raw = np.frombuffer(ctypes.string_at(p.planes[i], n), np.uint8)
+        return np.lib.stride_tricks.as_strided(raw, (rows, row_bytes), (p.stride[i], 1)).copy()
+    out = {"format": p.format, "log2_scale": p.log2_scale, "on_device": p.on_device, "y": plane(0, p.height, p.width)}
+    if p.format == PACKED_NV12:
+        out["cbcr"] = plane(1, p.height_C, 2 * p.width_C).reshape(p.height_C, p.width_C, 2)
+    else:
+        out["cb"], out["cr"] = plane(1, p.height_C, p.width_C), plane(2, p.height_C, p.width_C)
+    return out
+
+
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
-    ends with the frame's motion export (frame_motion)."""
+    carries the frame's motion export (frame_motion); with packed=(format, log2_scale) it ends with the frame's packed
+    output (frame_packed)."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -127,6 +168,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False):
             d = ctypes.c_void_p(dec)
             lib.edge264_free(ctypes.byref(d))
             raise RuntimeError("edge264_enable_motion: %s" % errno.errorcode.get(r, r))
+    if packed is not None:
+        r = lib.edge264_enable_packed(dec, packed[0], packed[1]) if hasattr(lib, "edge264_enable_packed") else errno.ENOTSUP
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_enable_packed: %s" % errno.errorcode.get(r, r))
     nal = base + 3 + (1 if data[2] == 0 else 0)
     frames, codes, f = [], [], Edge264Frame()
     drained = False
@@ -138,7 +185,7 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False):
             drained = True
         while lib.edge264_get_frame(dec, ctypes.byref(f), 0) == 0:
             frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ())
-                          + ((frame_motion(lib, dec, f),) if motion else ()))
+                          + ((frame_motion(lib, dec, f),) if motion else ()) + ((frame_packed(lib, dec, f),) if packed is not None else ()))
         if res == errno.ENOBUFS:
             if len(frames) == before:
                 break

@@ -180,6 +180,10 @@ typedef struct HostBuf {
 	uint8_t *motion;      /* the picture's motion export (records.h E264_MOTION_*), memory of the samples' kind; NULL without export */
 	void *motion_mbs;     /* the mbs allocation alloc_cb returned with it */
 	int motion_dev;       /* motion is device memory */
+	uint8_t *packed;      /* the picture's packed output (records.h e264_packed_layout), memory of the samples' kind; NULL without it */
+	void *packed_mbs;     /* the mbs allocation alloc_cb returned with it */
+	int packed_dev;       /* packed is device memory */
+	E264PackedDesc pk;    /* what the picture in the buffer was packed as (cropping rectangle of its sequence) */
 	int state;            /* 0 free, 1 attached to a decoded picture, 2 in the output queue, 3 handed out */
 	int borrowed;
 	int32_t frame_id;
@@ -226,7 +230,8 @@ struct Edge264Decoder {
 	int pending_release;               /* host buffer handed out without borrow, released at next decode_NAL */
 	int sync_output;                   /* E264_SYNC_OUTPUT=1: get_frame always waits for the device (the behaviour before round 2's last step; A/B switch) */
 	int motion;                        /* edge264_enable_motion: every output picture carries its motion export */
-	int slices_seen;                   /* a slice NAL unit has been decoded (edge264_enable_motion is refused from then on) */
+	int slices_seen;                   /* a slice NAL unit has been decoded (edge264_enable_motion / _packed are refused from then on) */
+	int packed, packed_format, packed_scale;   /* edge264_enable_packed: every output picture carries its packed output */
 	int block_output;                  /* the last decode_NAL asked the application to fetch frames (ENOBUFS, end of stream): get_frame waits for the device */
 	/* scratch: RBSP of the last non-slice NAL unit */
 	uint8_t *rbsp; size_t rbsp_cap;
@@ -262,6 +267,9 @@ typedef struct E264Backend {
 	 * export into `motion` (E264_MOTION_BYTES per macroblock), with slot_ids[s] the FrameId of frame slot s
 	 * (E264_MAX_SLOTS entries, -1 for an empty slot); *on_device tells whether `motion` is device memory. */
 	int  (*submit_motion)(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint8_t *motion, const int32_t *slot_ids, int *on_device, uint64_t *ticket);
+	/* packed output (include/edge264_packed.h); NULL: the backend has none.  submit with every optional output in one
+	 * struct (records.h E264Outputs): the error map, the motion export and the packed output, each left out when NULL. */
+	int  (*submit_outputs)(void *ctx, const E264PicDesc *pd, uint8_t *host_out, const E264Outputs *out, uint64_t *ticket);
 } E264Backend;
 const E264Backend *e264_default_backend(void);
 

@@ -16,6 +16,7 @@
 #include "dec.h"
 #include "h264_tables.h"
 #include "../../include/edge264_motion.h"
+#include "../../include/edge264_packed.h"
 
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
@@ -243,7 +244,30 @@ static void hostbuf_free(Edge264Decoder *d, HostBuf *hb) {
 		if (d->alloc_cb) d->free_cb(hb->motion, hb->motion_mbs, d->alloc_arg);
 		else d->be->host_free(d->be_ctx, hb->motion);
 	}
+	if (hb->packed) {
+		if (d->alloc_cb) d->free_cb(hb->packed, hb->packed_mbs, d->alloc_arg);
+		else d->be->host_free(d->be_ctx, hb->packed);
+	}
 	memset(hb, 0, sizeof(*hb));
+}
+/* what the pictures of the active sequence are packed as: the decoder's format and scale, the sequence's cropping rectangle */
+static E264PackedDesc packed_desc(const Edge264Decoder *d) {
+	const Edge264Frame *o = &d->out_fmt;
+	E264PackedDesc k = {d->packed_format, d->packed_scale, o->frame_crop_offsets[3], o->frame_crop_offsets[0],
+	                    d->w_mbs * 16 - o->frame_crop_offsets[3] - o->frame_crop_offsets[1], d->h_mbs * 16 - o->frame_crop_offsets[0] - o->frame_crop_offsets[2]};
+	return k;
+}
+/* a buffer beside the samples, of their memory kind: from the application's allocator, else from the backend's output
+ * mirrors (pinned host memory, device memory with E264B_OUTPUT=device) */
+static uint8_t *side_alloc(Edge264Decoder *d, size_t bytes, void **mbs) {
+	void *m = NULL;
+	if (d->alloc_cb) d->alloc_cb(&m, (unsigned)bytes, mbs, 0, ENOMEM, d->alloc_arg);
+	else {
+		pthread_mutex_lock(&d->be_lock);
+		m = d->be->host_alloc(d->be_ctx, bytes);
+		pthread_mutex_unlock(&d->be_lock);
+	}
+	return (uint8_t *)m;
 }
 static int hostbuf_acquire(Edge264Decoder *d) {
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state == 0 && d->hb[i].p) return i;
@@ -269,20 +293,11 @@ static int hostbuf_acquire(Edge264Decoder *d) {
 			pthread_mutex_unlock(&d->be_lock);
 			if (!hb->map) { hostbuf_free(d, hb); return -1; }
 		}
-		/* the motion export lives where the samples live: from the application's allocator, else from the backend's
-		 * output mirrors (pinned host memory, device memory with E264B_OUTPUT=device) */
-		if (d->motion) {
-			const size_t mbytes = (size_t)d->w_mbs * d->h_mbs * E264_MOTION_BYTES;
-			if (d->alloc_cb) {
-				void *m = NULL, *mbs = NULL;
-				d->alloc_cb(&m, (unsigned)mbytes, &mbs, 0, ENOMEM, d->alloc_arg);
-				hb->motion = (uint8_t *)m; hb->motion_mbs = mbs;
-			} else {
-				pthread_mutex_lock(&d->be_lock);
-				hb->motion = (uint8_t *)d->be->host_alloc(d->be_ctx, mbytes);
-				pthread_mutex_unlock(&d->be_lock);
-			}
-			if (!hb->motion) { hostbuf_free(d, hb); return -1; }
+		/* the motion export and the packed output live where the samples live */
+		if (d->motion && !(hb->motion = side_alloc(d, (size_t)d->w_mbs * d->h_mbs * E264_MOTION_BYTES, &hb->motion_mbs))) { hostbuf_free(d, hb); return -1; }
+		if (d->packed) {
+			const E264PackedDesc k = packed_desc(d);
+			if (!(hb->packed = side_alloc(d, (size_t)e264_packed_layout(&k).bytes, &hb->packed_mbs))) { hostbuf_free(d, hb); return -1; }
 		}
 		return i;
 	}
@@ -403,7 +418,11 @@ static int build_submit(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd, uint64
 	int r;
 	{
 		PROF_BEGIN;
-		if (d->motion) r = d->be->submit_motion(d->be_ctx, pd, hb->p, hb->map, hb->motion, pb->slot_ids, &hb->motion_dev, ticket);
+		if (d->packed) {   /* the picture is packed when it is reconstructed, like its samples are copied then */
+			hb->pk = packed_desc(d);
+			const E264Outputs o = {hb->map, hb->motion, pb->slot_ids, E264_MAX_SLOTS, &hb->motion_dev, hb->packed, hb->pk, &hb->packed_dev};
+			r = d->be->submit_outputs(d->be_ctx, pd, hb->p, &o, ticket);
+		} else if (d->motion) r = d->be->submit_motion(d->be_ctx, pd, hb->p, hb->map, hb->motion, pb->slot_ids, &hb->motion_dev, ticket);
 		else r = d->be->submit_maps ? d->be->submit_maps(d->be_ctx, pd, hb->p, hb->map, ticket) : d->be->submit(d->be_ctx, pd, hb->p, ticket);
 		PROF_END(2);
 	}
@@ -1306,5 +1325,31 @@ int edge264_get_motion(Edge264Decoder *d, const Edge264Frame *frame, Edge264Moti
 	out->mb_qp = m + E264_MOTION_QP * nmb;
 	out->width_mbs = d->w_mbs; out->height_mbs = d->h_mbs;
 	out->on_device = d->hb[i].motion_dev;
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* packed output (include/edge264_packed.h)                                                     */
+/* ------------------------------------------------------------------------------------------ */
+int edge264_enable_packed(Edge264Decoder *d, int format, int log2_scale) {
+	if (!d || (format != EDGE264_PACKED_I420 && format != EDGE264_PACKED_NV12) || log2_scale < 0 || log2_scale > 3) return EINVAL;
+	if (!d->be->submit_outputs) return ENOTSUP;
+	if (d->slices_seen) return EBUSY;   /* host buffers are created with the first picture: they would lack the packed one */
+	d->packed = 1; d->packed_format = format; d->packed_scale = log2_scale;
+	return 0;
+}
+
+int edge264_get_packed(Edge264Decoder *d, const Edge264Frame *frame, Edge264Packed *out) {
+	if (!d || !frame || !out) return EINVAL;
+	if (!d->packed) return ENOENT;
+	const int i = (int)(uintptr_t)frame->return_arg - 1;
+	if (i < 0 || i >= E264_MAX_HOSTBUFS || d->hb[i].state != 3 || !d->hb[i].packed) return EINVAL;
+	const HostBuf *hb = &d->hb[i];
+	const E264PackedLayout l = e264_packed_layout(&hb->pk);
+	memset(out, 0, sizeof(*out));
+	for (int p = 0; p < (hb->pk.format == E264_PACKED_NV12 ? 2 : 3); p++) { out->planes[p] = hb->packed + l.offset[p]; out->stride[p] = l.stride[p]; }
+	out->width = l.width; out->height = l.height; out->width_C = l.width_C; out->height_C = l.height_C;
+	out->format = hb->pk.format; out->log2_scale = hb->pk.log2_scale;
+	out->on_device = hb->packed_dev;
 	return 0;
 }

@@ -21,6 +21,7 @@
 #include "inter_kernels.cuh"
 #include "intra_kernels.cuh"
 #include "motion_kernels.cuh"
+#include "pack_kernels.cuh"
 extern "C" {
 #include "dec.h"
 }
@@ -44,6 +45,7 @@ struct E264bDevice {
 	uint8_t *d_frames;
 	uint8_t *d_maps;             /* [n_slots][nmb] error maps of the frame slots (written only for pictures with err_pic) */
 	uint8_t *d_motion;           /* [nmb * E264_MOTION_BYTES] motion export of the picture last submitted with one (allocated at the first) */
+	uint8_t *d_packed; size_t packed_cap;   /* packed output of the picture last submitted with one (allocated at the first, grown when a layout needs more) */
 	E264MbRec *h_recs[E264_MAX_SLOTS]; cudaEvent_t rec_up[E264_MAX_SLOTS]; bool rec_busy[E264_MAX_SLOTS];
 	Staging st[NSTAGE]; int stage, n_stage;
 	unsigned *d_sync;            /* synchronisation words, layout SYNC_* in recon_kernels.cuh */
@@ -75,6 +77,8 @@ static void free_geometry(E264bDevice *c) {
 	c->d_maps = NULL;
 	if (c->d_motion) cudaFree(c->d_motion);
 	c->d_motion = NULL;
+	if (c->d_packed) cudaFree(c->d_packed);
+	c->d_packed = NULL; c->packed_cap = 0;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { if (c->h_recs[i]) cudaFreeHost(c->h_recs[i]); c->h_recs[i] = NULL; c->rec_busy[i] = false; }
 	for (int i = 0; i < NSTAGE; i++) {
 		Staging *s = &c->st[i];
@@ -109,7 +113,7 @@ extern "C" int e264b_create(E264bDevice **out) {
 		}
 	}
 	E264bDevice *c = new E264bDevice();
-	c->dev = 0; c->stream = 0; memset(&c->g, 0, sizeof(c->g)); c->n_slots = 0; c->nmb = 0; c->coef_cap = 0; c->d_frames = NULL; c->d_maps = NULL; c->d_motion = NULL;
+	c->dev = 0; c->stream = 0; memset(&c->g, 0, sizeof(c->g)); c->n_slots = 0; c->nmb = 0; c->coef_cap = 0; c->d_frames = NULL; c->d_maps = NULL; c->d_motion = NULL; c->d_packed = NULL; c->packed_cap = 0;
 	memset(c->h_recs, 0, sizeof(c->h_recs)); memset(c->rec_busy, 0, sizeof(c->rec_busy)); memset(c->st, 0, sizeof(c->st)); c->stage = 0; c->d_sync = NULL; c->epoch = 0; c->tick_seq = 0;
 	c->launches = c->h2d_bytes = c->d2h_bytes = 0;
 	c->dev = dev;
@@ -319,11 +323,68 @@ static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd
 	return 0;
 }
 
+/* the packed output of the picture in frame slot pd->dst_slot into d_packed: one launch over all planes */
+template <int K> static void launch_pack(E264bDevice *c, int format, int blocks, const PackArgs &A) {
+	if (format == E264_PACKED_NV12) e264_pack_kernel<K, E264_PACKED_NV12><<<blocks, PACK_THREADS, 0, c->stream>>>(A);
+	else e264_pack_kernel<K, E264_PACKED_I420><<<blocks, PACK_THREADS, 0, c->stream>>>(A);
+}
+static int pack_picture(E264bDevice *c, const E264PicDesc *pd, const E264PackedDesc *pk, const E264PackedLayout &L) {
+	const uint8_t *slot = c->d_frames + (size_t)pd->dst_slot * pd->frame_bytes;
+	const bool nv12 = pk->format == E264_PACKED_NV12;
+	const int n = 1 << pk->log2_scale;
+	PackArgs A; memset(&A, 0, sizeof(A));
+	int blocks = 0;
+	for (int i = 0; i < (nv12 ? 2 : 3); i++) {
+		PackPlane &P = A.p[i];
+		if (i == 0) { P.src = slot + (size_t)pk->top * pd->stride_y + pk->left; P.src_stride = pd->stride_y; P.w = pk->width; P.h = pk->height; }
+		else {
+			P.src = slot + pd->plane_y + (size_t)(pk->top >> 1) * pd->stride_c + (pk->left >> 1) + (i == 2 ? pd->stride_c >> 1 : 0);
+			P.src_stride = pd->stride_c; P.w = pk->width >> 1; P.h = pk->height >> 1;
+		}
+		P.dst = c->d_packed + L.offset[i]; P.dst_stride = L.stride[i];
+		const int words = ((P.w + n - 1) / n + 3) / 4, rows = (P.h + n - 1) / n;
+		P.bx = (words + 31) / 32; P.first = blocks;
+		blocks += P.bx * ((rows + PACK_ROWS - 1) / PACK_ROWS);
+	}
+	if (nv12) A.p[2].first = blocks;
+	A.cr_off = pd->stride_c >> 1;
+	switch (pk->log2_scale) {
+	case 0: launch_pack<0>(c, pk->format, blocks, A); break;
+	case 1: launch_pack<1>(c, pk->format, blocks, A); break;
+	case 2: launch_pack<2>(c, pk->format, blocks, A); break;
+	default: launch_pack<3>(c, pk->format, blocks, A); break;
+	}
+	c->launches++;
+	CK(cudaGetLastError());
+	return 0;
+}
+
+static int is_device_memory(const void *p) {
+	cudaPointerAttributes a;
+	const int dev = cudaPointerGetAttributes(&a, p) == cudaSuccess && a.type == cudaMemoryTypeDevice;
+	cudaGetLastError();
+	return dev;
+}
+
 extern "C" int e264b_submit(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint64_t *ticket) { return e264b_submit_maps(c, pd, host_out, NULL, ticket); }
 extern "C" int e264b_submit_maps(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint64_t *ticket) {
 	return e264b_submit_motion(c, pd, host_out, host_map, NULL, NULL, 0, NULL, ticket);
 }
 extern "C" int e264b_submit_motion(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, uint8_t *host_map, uint8_t *motion, const int32_t *slot_ids, int n_ids, int *on_device, uint64_t *ticket) {
+	E264Outputs o; memset(&o, 0, sizeof(o));
+	o.map = host_map; o.motion = motion; o.slot_ids = slot_ids; o.n_ids = n_ids; o.motion_on_device = on_device;
+	return e264b_submit_outputs(c, pd, host_out, &o, ticket);
+}
+extern "C" int e264b_submit_outputs(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, const E264Outputs *o, uint64_t *ticket) {
+	uint8_t *const host_map = o->map, *const motion = o->motion, *const packed = o->packed;
+	const int32_t *const slot_ids = o->slot_ids; const int n_ids = o->n_ids;
+	E264PackedLayout pl; memset(&pl, 0, sizeof(pl));
+	if (packed) {
+		const E264PackedDesc *k = &o->pk;
+		if ((k->format != E264_PACKED_I420 && k->format != E264_PACKED_NV12) || k->log2_scale < 0 || k->log2_scale > 3 || ((k->left | k->top | k->width | k->height) & 1) ||
+		    k->left < 0 || k->top < 0 || k->width < 2 || k->height < 2 || k->left + k->width > pd->width_mbs * 16 || k->top + k->height > pd->height_mbs * 16) return -1;
+		pl = e264_packed_layout(k);
+	}
 	CK(cudaSetDevice(c->dev));
 	if (motion && (n_ids < 0 || n_ids > MOTION_MAX_SLOTS)) return -1;
 	if (pd->staging < 0 || pd->staging >= c->n_stage) return -1;
@@ -361,7 +422,18 @@ extern "C" int e264b_submit_motion(E264bDevice *c, const E264PicDesc *pd, uint8_
 		c->launches++;
 		CK(cudaGetLastError());
 		CK(cudaMemcpyAsync(motion, c->d_motion, bytes, cudaMemcpyDefault, c->stream)); c->d2h_bytes += bytes;
-		if (on_device) { cudaPointerAttributes a; *on_device = cudaPointerGetAttributes(&a, motion) == cudaSuccess && a.type == cudaMemoryTypeDevice; cudaGetLastError(); }
+		if (o->motion_on_device) *o->motion_on_device = is_device_memory(motion);
+	}
+	if (packed) {   /* the packed output, from the finished frame slot; through a scratch like the motion export, so that the kernel's
+	                 * stores are aligned whatever memory the application's alloc_cb returned */
+		if ((size_t)pl.bytes > c->packed_cap) {
+			if (c->d_packed) CK(cudaFree(c->d_packed));   /* waits for the copy of the picture before */
+			c->d_packed = NULL; c->packed_cap = 0;
+			CK(cudaMalloc(&c->d_packed, pl.bytes)); c->packed_cap = pl.bytes;
+		}
+		if (pack_picture(c, pd, &o->pk, pl)) return -1;
+		CK(cudaMemcpyAsync(packed, c->d_packed, pl.bytes, cudaMemcpyDefault, c->stream)); c->d2h_bytes += pl.bytes;
+		if (o->packed_on_device) *o->packed_on_device = is_device_memory(packed);
 	}
 	if (c->keep) {
 		KeptPic k; k.pd = *pd;
@@ -726,8 +798,9 @@ static void be_pinned_free(void *ctx, void *p) { e264b_pinned_free((E264bDevice 
 static int be_submit_motion(void *ctx, const E264PicDesc *pd, uint8_t *out, uint8_t *map, uint8_t *motion, const int32_t *ids, int *on_device, uint64_t *t) {
 	return e264b_submit_motion((E264bDevice *)ctx, pd, out, map, motion, ids, E264_MAX_SLOTS, on_device, t);
 }
+static int be_submit_outputs(void *ctx, const E264PicDesc *pd, uint8_t *out, const E264Outputs *o, uint64_t *t) { return e264b_submit_outputs((E264bDevice *)ctx, pd, out, o, t); }
 static_assert(E264_MAX_SLOTS <= MOTION_MAX_SLOTS, "the motion kernel's FrameId table holds every frame slot");
 static const E264Backend cuda_backend = {"cuda-sm_90a", be_create, be_destroy, be_configure, be_host_alloc, be_host_free, be_acquire, be_submit, be_wait, be_fill, be_poll, be_submit_maps, be_pinned_alloc, be_pinned_free,
-                                         be_submit_motion};
+                                         be_submit_motion, be_submit_outputs};
 extern "C" const E264Backend *e264_default_backend(void) { return &cuda_backend; }
 extern "C" E264bDevice *e264b_of_decoder(Edge264Decoder *d) { return d ? (E264bDevice *)d->be_ctx : NULL; }

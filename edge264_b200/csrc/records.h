@@ -137,6 +137,45 @@ typedef struct E264PicDesc {
  *   mb_qp         E264_MOTION_QP * nmb    uint8 [height_mbs][width_mbs] */
 enum { E264_MOTION_MV = 0, E264_MOTION_REF = 128, E264_MOTION_TYPE = 160, E264_MOTION_QP = 161, E264_MOTION_BYTES = 162 };
 
+/* The packed output of one picture (include/edge264_packed.h): the cropped picture as I420 or NV12, box-downscaled by
+ * 1 << log2_scale, in one buffer.  E264PackedDesc says what to pack, e264_packed_layout where every plane goes: sizes are
+ * ceil(cropped size / scale), a row stride is the row's bytes rounded up to 64, a plane starts on a multiple of 256. */
+enum { E264_PACKED_I420 = 0, E264_PACKED_NV12 = 1 };
+typedef struct E264PackedDesc {
+	int32_t format, log2_scale;         /* E264_PACKED_*, 0..3 */
+	int32_t left, top, width, height;   /* the cropping rectangle inside the coded picture, luma samples (all even: 4:2:0 frames) */
+} E264PackedDesc;
+typedef struct E264PackedLayout {
+	int32_t width, height, width_C, height_C;   /* samples per plane after cropping and scaling */
+	int32_t stride[3], offset[3];               /* I420: Y, Cb, Cr; NV12: Y, interleaved CbCr, unused (0) */
+	int32_t bytes;                              /* size of the buffer */
+} E264PackedLayout;
+static inline E264PackedLayout e264_packed_layout(const E264PackedDesc *p) {
+	const int n = 1 << p->log2_scale;
+	E264PackedLayout l;
+	l.width = (p->width + n - 1) >> p->log2_scale; l.height = (p->height + n - 1) >> p->log2_scale;
+	l.width_C = ((p->width >> 1) + n - 1) >> p->log2_scale; l.height_C = ((p->height >> 1) + n - 1) >> p->log2_scale;
+	l.stride[0] = (l.width + 63) & ~63;
+	l.stride[1] = ((p->format == E264_PACKED_NV12 ? 2 * l.width_C : l.width_C) + 63) & ~63;
+	l.stride[2] = p->format == E264_PACKED_NV12 ? 0 : l.stride[1];
+	l.offset[0] = 0;
+	l.offset[1] = (l.stride[0] * l.height + 255) & ~255;
+	l.offset[2] = p->format == E264_PACKED_NV12 ? 0 : (l.offset[1] + l.stride[1] * l.height_C + 255) & ~255;
+	l.bytes = (p->format == E264_PACKED_NV12 ? l.offset[1] + l.stride[1] * l.height_C : l.offset[2] + l.stride[2] * l.height_C);
+	l.bytes = (l.bytes + 255) & ~255;
+	return l;
+}
+
+/* What a submit may produce besides the samples; a NULL pointer leaves that output out (no launch, no copy, no
+ * allocation for it).  map: the error map, copied when pd->err_pic.  motion: the motion export, slot_ids[s] the FrameId
+ * of frame slot s for s < n_ids, -1 elsewhere.  packed: the packed output described by pk.  The *_on_device words (may be
+ * NULL) receive whether that destination is device memory. */
+typedef struct E264Outputs {
+	uint8_t *map;
+	uint8_t *motion; const int32_t *slot_ids; int32_t n_ids; int *motion_on_device;
+	uint8_t *packed; E264PackedDesc pk; int *packed_on_device;
+} E264Outputs;
+
 /* Host-visible staging of one picture, handed out by the backend (pinned memory for the CUDA backend): the parser
  * writes records, levels and slice records straight into it; intra_list receives the addresses of the picture's intra
  * macroblocks in raster order (the device schedules them from it). */

@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-struct E264MbRec; struct E264SliceRec; struct E264PicDesc; struct E264Staging; struct Edge264Decoder;
+struct E264MbRec; struct E264SliceRec; struct E264PicDesc; struct E264Staging; struct E264Outputs; struct Edge264Decoder;
 typedef struct E264bDevice E264bDevice;
 
 int   e264b_create(E264bDevice **out);              /* device = $E264B_DEVICE (default 0); fails without a GPU */
@@ -43,6 +43,11 @@ int   e264b_submit_maps(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t
  * memory.  With motion NULL it is e264b_submit_maps: no launch, no copy. */
 int   e264b_submit_motion(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, uint8_t *host_map, uint8_t *motion,
                           const int32_t *slot_ids, int n_ids, int *on_device, uint64_t *ticket);
+/* The one submit the three above are thin callers of: `out` (struct E264Outputs of edge264_b200/csrc/records.h) names the
+ * optional outputs, each left out when its pointer is NULL: the error map, the motion export, and the packed output
+ * (include/edge264_packed.h: the cropped picture as I420 or NV12, optionally box-downscaled, written by e264_pack_kernel
+ * with the layout of e264_packed_layout; one launch and one copy of that many bytes per picture). */
+int   e264b_submit_outputs(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, const struct E264Outputs *out, uint64_t *ticket);
 int   e264b_wait(E264bDevice *dev, uint64_t ticket);
 int   e264b_poll(E264bDevice *dev, uint64_t ticket);          /* 0 complete, EAGAIN still on the device, < 0 device error */
 int   e264b_fill_slot(E264bDevice *dev, int slot, int luma, int chroma);   /* and the slot's error map to all 100 */
