@@ -57,15 +57,18 @@ __device__ __forceinline__ void mc_load_chroma(const uint8_t *plane, int stride,
 	}
 }
 
-/* 8.4.2.3 on four packed samples in ONE form: ((a * wa + b * wb + rnd) >> sh) + o, clipped.  Explicit or implicit
- * bi-prediction: wa = w0, wb = w1, rnd = 2^logWD, sh = logWD + 1; explicit weighting of a single prediction: wa = w, wb = 0,
- * rnd = 2^(logWD-1) (0 when logWD = 0), sh = logWD (reference edge264_inter.c:1140-1180 keeps five variants). */
+/* 8.4.2.3 on four packed samples in ONE form: (sat16(a * wa + b * wb + rnd) >> sh) + o, clipped.  Implicit bi-prediction:
+ * wa = w0, wb = w1, rnd = 2^logWD, sh = logWD + 1, o = 0; explicit bi-prediction: the same with the offsets folded into
+ * rnd = ((o0 + o1 + 1) | 1) << logWD and o = 0, saturated to int16 as the reference does (edge264_inter.c:17-29,
+ * :1176-1178; it differs from the standard only at logWD 7, oracle/port_recon.c wp_bi); explicit weighting of a single
+ * prediction: wa = w, wb = 0, rnd = 2^(logWD-1) (0 when logWD = 0), sh = logWD.  Only explicit bi-prediction can reach the
+ * saturation (reference edge264_inter.c:1140-1180 keeps five variants). */
 __device__ __forceinline__ uint32_t wp_word(uint32_t a, uint32_t b, int wa, int wb, int rnd, int sh, int o) {
 	uint32_t r = 0;
 #pragma unroll
 	for (int k = 0; k < 4; k++) {
 		const int pa = (a >> (8 * k)) & 255, pb = (b >> (8 * k)) & 255;
-		r |= (uint32_t)mc_clip255(((pa * wa + pb * wb + rnd) >> sh) + o) << (8 * k);
+		r |= (uint32_t)mc_clip255((min(max(pa * wa + pb * wb + rnd, -32768), 32767) >> sh) + o) << (8 * k);
 	}
 	return r;
 }
@@ -258,7 +261,7 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 #pragma unroll
 						for (int k = 0; k < 2; k++) {
 							const int c = k ? 1 + h : 0, lw = k ? sr->chroma_log2_wd : sr->luma_log2_wd;
-							if (bi && wpm == WP_EXPLICIT) { wa[k] = sr->wp_w[0][r0 & 15][c]; wb[k] = sr->wp_w[1][r1 & 15][c]; o[k] = (sr->wp_o[0][r0 & 15][c] + sr->wp_o[1][r1 & 15][c] + 1) >> 1; sh[k] = lw + 1; rnd[k] = 1 << lw; }
+							if (bi && wpm == WP_EXPLICIT) { wa[k] = sr->wp_w[0][r0 & 15][c]; wb[k] = sr->wp_w[1][r1 & 15][c]; o[k] = 0; sh[k] = lw + 1; rnd[k] = ((sr->wp_o[0][r0 & 15][c] + sr->wp_o[1][r1 & 15][c] + 1) | 1) * (1 << lw); }
 							else if (bi) { wb[k] = sr->implicit_w1[r0 & 15][r1 & 15]; wa[k] = 64 - wb[k]; o[k] = 0; sh[k] = 6; rnd[k] = 32; }
 							else { wa[k] = sr->wp_w[ll][ri][c]; wb[k] = 0; o[k] = sr->wp_o[ll][ri][c]; sh[k] = lw; rnd[k] = lw >= 1 ? 1 << (lw - 1) : 0; }
 						}

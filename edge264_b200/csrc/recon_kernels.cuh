@@ -204,7 +204,15 @@ static_assert(offsetof(E264SliceRec, scaling4x4) % 8 == 0 && offsetof(E264SliceR
               "idct4x4 loads a 4x4 scaling list as two 8-byte words, residual_stage a row of an 8x8 list as one");
 __device__ __noinline__ void idct4x4(const int16_t *c, bool have_levels, const uint8_t *scaling, int qp, bool dc_override, int dc, int16_t *dst, int dstride) {
 	int d[16];
-	if (have_levels) {
+	if (!have_levels) {   /* DC only: (dc + 32) >> 6 truncated to int16, as the reference's add_dc4x4 (oracle/port_recon.c port_dc4x4) */
+		const int16_t v = dc_override ? (int16_t)((dc + 32) >> 6) : 0;
+#pragma unroll
+		for (int i = 0; i < 4; i++)
+#pragma unroll
+			for (int j = 0; j < 4; j++) dst[i * dstride + j] = v;
+		return;
+	}
+	{
 		uint4 a = *(const uint4 *)c, b = *((const uint4 *)c + 1);   /* c points into the TMA-staged shared copy */
 		int16_t lv[16];
 		*(uint4 *)lv = a; *(uint4 *)(lv + 8) = b;
@@ -222,9 +230,6 @@ __device__ __noinline__ void idct4x4(const int16_t *c, bool have_levels, const u
 				int ls = (int)((sw[i] >> (8 * j)) & 255u) * nrm;
 				d[i * 4 + j] = (int)(((unsigned)(lv[i * 4 + j] * ls) << sh) + 8u) >> 4;
 			}
-	} else {
-#pragma unroll
-		for (int i = 0; i < 16; i++) d[i] = 0;
 	}
 	if (dc_override) d[0] = dc;
 	int f[16];

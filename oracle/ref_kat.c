@@ -1,7 +1,8 @@
 /* oracle/ref_kat.c — TEST INFRASTRUCTURE (build container only).  Includes the reference's intra and inter
  * sources the way its own edge264_check.c:20-22 does, and
- *   ref_kat fuzz     differential fuzz of the reference's decode_inter_luma / decode_inter_chroma against
- *                    the plain-C restatement (oracle/port_recon.c), all 48 luma modes, random + extreme sources
+ *   ref_kat fuzz     differential fuzz of the reference's decode_inter_luma against the plain-C restatement
+ *                    (oracle/port_recon.c), all 48 luma modes, random + extreme sources (decode_inter_chroma is not
+ *                    fuzzed here: chroma interpolation is pinned through whole streams, tests/test_limits.py among them)
  *   ref_kat residual differential fuzz of the reference's add_idct4x4 / add_idct8x8 / transform_dc4x4 / transform_dc2x2
  *                    (edge264_residual.c:108-538) against port_idct4x4 / port_idct8x8 / port_luma_dc / port_chroma_dc:
  *                    random QP 0..51, random and flat scaling lists, intra/inter lists, conformant-range and extreme levels

@@ -19,7 +19,7 @@
 
 void port_recon_picture(uint8_t *frames, const E264PicDesc *pd, const E264MbRec *recs, const int16_t *coefs, const E264SliceRec *slices);
 int port_boundary_strength(const E264MbRec *p, int bp, const E264MbRec *q, int bq, int mb_edge);
-extern long port_cov_residual[5];
+extern long port_cov_residual[6], port_cov_wp_bi_sat16;
 
 /* ---- the device, through the product library's C ABI (include/e264b_recon.h) ---- */
 static struct {
@@ -60,7 +60,7 @@ enum {
 	C_BS,   /* 30 entries: [left, top, internal][t4x4, t8x8][bS 0..4] */
 	C_FOFF_M12 = C_BS + 30, C_FOFF_P12, C_IDC0, C_IDC1, C_IDC2, C_SLICES64,
 	C_INTRA_COMBOS, C_IPCM, C_CONCEAL_INTER, C_CONCEAL_INTRA,
-	C_FRAC_0, C_FRAC_1, C_FRAC_BELOW, C_FRAC_AT, C_FRAC_ABOVE, C_FRAC_ALL, C_PICTURES, C_N
+	C_FRAC_0, C_FRAC_1, C_FRAC_BELOW, C_FRAC_AT, C_FRAC_ABOVE, C_FRAC_ALL, C_WP_LWD7_BRIGHT, C_PICTURES, C_N
 };
 static long cov[C_N];
 static uint64_t qp_seen[3];
@@ -119,6 +119,16 @@ static void draw_slice(E264SliceRec *s, int n_slots) {
 		if (lwd == 7 && pct(30)) w = 128;      /* the inferred default at logWD 7 */
 		s->wp_w[l][i][k] = (int16_t)w;
 		s->wp_o[l][i][k] = (int16_t)(pct(30) ? pick((const int[]){-128, 127, 0}, 3) : rnd(256) - 128);
+	}
+	if (pct(15)) {   /* conforming explicit bi-prediction at logWD 7 (w0 + w1 = 127, positive offsets): on bright sources the
+	                  * weighted sum plus the offset term leaves int16, which the reference saturates (port_recon.c wp_bi) */
+		int a = 64 + rnd(64);
+		s->wp_mode = WP_EXPLICIT; s->luma_log2_wd = s->chroma_log2_wd = 7;
+		for (int l = 0; l < 2; l++) for (int i = 0; i < 16; i++) for (int k = 0; k < 3; k++) {
+			s->wp_w[l][i][k] = (int16_t)(l ? 127 - a : a);
+			s->wp_o[l][i][k] = (int16_t)(1 + rnd(127));
+		}
+		cov[C_WP_LWD7_BRIGHT]++;
 	}
 	for (int i = 0; i < 16; i++) for (int j = 0; j < 16; j++) s->implicit_w1[i][j] = (int16_t)(pct(40) ? pick((const int[]){-64, 128, 32}, 3) : rnd(193) - 64);
 	int kind = rnd(4);
@@ -468,11 +478,12 @@ int main(int argc, char **argv) {
 		if (i >= C_BS + 30 && i < C_FOFF_M12) continue;
 		static const char *tail[] = {"filter_offset_-12", "filter_offset_12", "deblock_idc_0", "deblock_idc_1", "deblock_idc_2", "slices_64",
 			"intra_mode_availability_pairs", "ipcm", "conceal_inter", "conceal_intra", "intra_fraction_0", "intra_fraction_1",
-			"intra_fraction_below_half", "intra_fraction_half", "intra_fraction_above_half", "intra_fraction_all", "pictures"};
+			"intra_fraction_below_half", "intra_fraction_half", "intra_fraction_above_half", "intra_fraction_all", "explicit_bi_logwd7_bright", "pictures"};
 		printf("cov %s %ld\n", i < C_BS ? names[i] : tail[i - C_FOFF_M12], cov[i]);
 	}
-	static const char *res[5] = {"sat16_4x4", "wrap_8x8_div_lt6", "wrap_8x8_div_ge6", "wrap_luma_dc32", "chroma_dc_qpc39"};
-	for (int i = 0; i < 5; i++) printf("cov %s %ld\n", res[i], port_cov_residual[i]);
+	static const char *res[6] = {"sat16_4x4", "wrap_8x8_div_lt6", "wrap_8x8_div_ge6", "wrap_luma_dc32", "chroma_dc_qpc39", "wrap16_dc_only"};
+	for (int i = 0; i < 6; i++) printf("cov %s %ld\n", res[i], port_cov_residual[i]);
+	printf("cov wp_bi_sat16 %ld\n", port_cov_wp_bi_sat16);
 	printf("%d pictures, %d failing seeds\n", total, fails);
 	return fails ? 1 : 0;
 }

@@ -23,6 +23,13 @@
  *          [--dpb] [--mmco5] [--poc-type 0|1|2]  (with --gop IP / IPB: reference-list modification to short- and long-term
  *                                           pictures, memory-management operations 1,2,3,4,6, long-term IDR,
  *                                           4-bit frame_num wrap-around; picture order count types 1 and 2)
+ *   the standard's limits (tests/test_limits.py; none of these changes a stream written without them):
+ *          [--wp-range full]                (explicit weights over -128..127 with both ends forced now and then, offsets over
+ *                                            -128..127, logWD 0..7; B pairs at -128 <= w0 + w1 <= (logWD 7 ? 127 : 128))
+ *          [--qp-walk]                      (mb_qp_delta over -26..25, QP_Y wrapping modulo 52 both ways, slice QPs 0 and 51)
+ *          [--cqp-offset A,B]               (chroma_qp_index_offset A and second_chroma_qp_index_offset B in every PPS)
+ *          [--levels big]                   (levels up to the 8-bit bound -32768..32767: CAVLC escapes, long CABAC suffixes)
+ *          [--pcm-extreme]                  (PCM macroblocks with 0/255 steps, full-range ramps, checkers and random bits)
  */
 #define E264_ENCODER
 #include <stdio.h>
@@ -49,6 +56,7 @@ typedef struct GenState {
 	int drift[2];           /* per-picture global motion */
 	int cur_is_b;
 	int direct4x4, nonref_p, extra_nals, bref, crop_left, crop_right, crop_top, mixed, ps_update, dpb_mode, mmco5, poc_type, max_long_idx_plus1, stat_rplm, stat_mmco[7], stat_idr_long;   /* --dpb: list modification + memory-management stress on I P P P streams; --poc-type 0|1|2 */
+	int wp_full, qp_walk, cqp_fixed, cqp[2], levels_big, pcm_extreme;   /* the standard's limits (file header) */
 } GenState;
 
 static inline uint64_t rnd64(GenState *g) { uint64_t x = g->rng; x ^= x >> 12; x ^= x << 25; x ^= x >> 27; g->rng = x; return x * 0x2545F4914F6CDD1Dull; }
@@ -121,12 +129,12 @@ static void write_pps(GenState *g, ByteBuf *out, int id, int init_qp) {
 	bw_ue(&w, g->refs - 1 < 0 ? 0 : g->refs - 1); bw_ue(&w, 0);      /* default active refs: l0 = refs, l1 = 1 */
 	bw_u(&w, 1, g->wp_p); bw_u(&w, 2, g->wp_b);
 	bw_se(&w, init_qp - 26); bw_se(&w, 0);
-	bw_se(&w, rnd(g, 9) - 4);
+	bw_se(&w, g->cqp_fixed ? g->cqp[0] : rnd(g, 9) - 4);
 	bw_u(&w, 1, 1); bw_u(&w, 1, 0); bw_u(&w, 1, 0);
 	bw_u(&w, 1, g->t8x8_mode);
 	bw_u(&w, 1, g->scaling >= 2);
 	if (g->scaling >= 2) put_scaling_matrix(g, &w, 6 + 2 * g->t8x8_mode);
-	bw_se(&w, rnd(g, 9) - 4);
+	bw_se(&w, g->cqp_fixed ? g->cqp[1] : rnd(g, 9) - 4);
 	bw_trailing(&w);
 	e264_emit_nal(out, 3, 8, w.buf, w.pos / 8); free(w.buf);
 }
@@ -134,6 +142,16 @@ static void write_pps(GenState *g, ByteBuf *out, int id, int init_qp) {
 /* ------------------------------------------------------------------------------------------ */
 /* macroblock chooser                                                                           */
 /* ------------------------------------------------------------------------------------------ */
+/* --levels big: magnitudes spread over every power of two up to the 8-bit bound (7.4.5.3.2: -2^15 .. 2^15-1), so that CAVLC
+ * takes level_prefix 15, 16 and above and CABAC long Exp-Golomb suffixes; now and then exactly -32768 or 32767 */
+static int big_level(GenState *g) {
+	int r = rnd(g, 16);
+	if (r == 0) return -32768;
+	if (r == 1) return 32767;
+	int b = rnd(g, 16), m = (1 << b) + rnd(g, 1 << b);   /* [2^b, 2^(b+1)) */
+	if (m > 32767) m = 32767;
+	return rnd(g, 2) ? -m : m;
+}
 static void gen_block(GenState *g, int16_t *blk, int n, int first, const uint8_t *scan, int rich) {
 	/* a few low-frequency-biased coefficients */
 	int cnt = 1 + rnd(g, rich ? 6 : 3);
@@ -141,6 +159,7 @@ static void gen_block(GenState *g, int16_t *blk, int n, int first, const uint8_t
 		int k = first + rnd(g, 1 + rnd(g, n - first));
 		int lv = laplace(g, 2); if (lv == 0) lv = rnd(g, 2) ? 1 : -1;
 		if (rnd(g, 40) == 0) lv *= 1 + rnd(g, 12);
+		if (g->levels_big && rnd(g, 4) == 0) lv = big_level(g);
 		blk[scan[k]] = (int16_t)lv;
 	}
 }
@@ -201,6 +220,23 @@ static void gen_mv(GenState *g, SliceCtx *s, int x4, int y4, int w4, int h4, int
 	out[0] = (int16_t)mvx; out[1] = (int16_t)mvy;
 }
 
+/* --pcm-extreme: one 16x16 luma and two 8x8 chroma planes of a PCM macroblock at the ends of the sample range, so that the
+ * intra predictors (8x8 reference filter, plane, DC) and the interpolation filters of the next pictures read extreme
+ * neighbourhoods: a 0/255 step, a ramp over the full range, a 0/255 checker, or random bits (bytes or 0/255) */
+static void gen_pcm_extreme(GenState *g, uint8_t *pcm) {
+	int kind = rnd(g, 4), dir = rnd(g, 3), flip = rnd(g, 2) ? 255 : 0, at = 1 + rnd(g, 15), period = 1 + rnd(g, 2), bytes = rnd(g, 2);
+	for (int i = 0; i < 384; i++) {
+		int n = i < 256 ? 16 : 8, j = i < 256 ? i : (i - 256) & 63, x = j % n, y = j / n;
+		int t = dir == 0 ? x : dir == 1 ? y : (x + y) / 2;   /* position across the pattern, 0..n-1 */
+		int v;
+		if (kind == 0) v = t * 16 / n < at ? 0 : 255;
+		else if (kind == 1) v = t * 255 / (n - 1);
+		else if (kind == 2) v = ((x / period + y / period) & 1) ? 255 : 0;
+		else v = bytes ? rnd(g, 256) : rnd(g, 2) * 255;
+		pcm[i] = (uint8_t)(v ^ flip);
+	}
+}
+
 static void gen_choose_intra(GenState *g, SliceCtx *s, MbSyn *m, int base) {
 	int r = rnd(g, 100);
 	int un16 = sx_unavail16(s);
@@ -213,7 +249,8 @@ static void gen_choose_intra(GenState *g, SliceCtx *s, MbSyn *m, int base) {
 			int phx = rnd(g, 3), phy = rnd(g, 3);
 			for (int i = 0; i < 256; i++) m->pcm[i] = (uint8_t)((((((i & 15) + phx) % 3 == 1) == ((((i >> 4) + phy) % 3) == 1)) ? 255 : 0) ^ (rnd(g, 32) ? 0 : rnd(g, 4)));
 			for (int i = 256; i < 384; i++) m->pcm[i] = (uint8_t)((((i & 7) + ((i >> 3) & 7) + phx) & 1) ? 255 : 0);
-		} else
+		} else if (g->pcm_extreme) gen_pcm_extreme(g, m->pcm);
+		else
 		for (int i = 0; i < 384; i++) m->pcm[i] = (uint8_t)(rnd(g, 8) ? v + rnd(g, 9) - 4 : rnd(g, 256));
 		return;
 	}
@@ -236,8 +273,12 @@ static void gen_choose_intra(GenState *g, SliceCtx *s, MbSyn *m, int base) {
 static void gen_choose_mb(GenState *g, SliceCtx *s, MbSyn *m, int allow_skip) {
 	memset(m, 0, sizeof(*m));
 	int st = s->slice_type;
-	m->qp_delta = rnd(g, 3) == 0 ? rnd(g, 5) - 2 : 0;
-	{   /* keep QP inside [qp0-8, qp0+10] (touches both 8x8 dequant branches when qp0 ~ 30) */
+	if (g->qp_walk) {   /* --qp-walk: any delta of -26..25, often landing on QP_Y 0 or 51; QP_Y wraps modulo 52 (7.4.5) */
+		int r = rnd(g, 8), d = r == 0 ? -s->qp : r == 1 ? 51 - s->qp : r < 5 ? rnd(g, 52) - 26 : 0;
+		m->qp_delta = d > 25 ? d - 52 : d < -26 ? d + 52 : d;
+	} else {
+		m->qp_delta = rnd(g, 3) == 0 ? rnd(g, 5) - 2 : 0;
+		/* keep QP inside [qp0-8, qp0+10] (touches both 8x8 dequant branches when qp0 ~ 30) */
 		int q = s->qp + m->qp_delta;
 		if (q < g->qp0 - 8 || q > g->qp0 + 10 || q < 0 || q > 51) m->qp_delta = 0;
 	}
@@ -305,6 +346,33 @@ static void gen_choose_mb(GenState *g, SliceCtx *s, MbSyn *m, int allow_skip) {
 /* pictures                                                                                     */
 /* ------------------------------------------------------------------------------------------ */
 typedef struct PicPlan { int type; int idr; int is_ref; int frame_num; int poc; } PicPlan;   /* type: 0 P, 1 B, 2 I */
+
+/* --wp-range full: one picture's explicit weight table.  Weights -128..127 (both ends forced now and then), offsets
+ * -128..127, luma and chroma logWD 0..7; about a quarter of the entries take the inferred 2^logWD and offset 0 (their flag is
+ * then 0, so 128 at logWD 7 in P pictures).  B pictures (7.4.3.2): every weight is coded at logWD 7, and each list-1 weight
+ * keeps -128 <= w0 + w1 <= (logWD == 7 ? 127 : 128) with every list-0 weight in use, now and then at either bound. */
+static int wp_full_value(GenState *g, int mid) { int r = rnd(g, 8); return r == 0 ? -128 : r == 1 ? 127 : r == 2 ? mid : rnd(g, 256) - 128; }
+static void gen_wp_full(GenState *g, int is_b, int n0, int *lwd, int *cwd, int16_t w[2][16][3], int16_t o[2][16][3]) {
+	*lwd = rnd(g, 8); *cwd = rnd(g, 8);
+	for (int l = 0; l < 2; l++) for (int i = 0; i < 16; i++) for (int c = 0; c < 3; c += c ? 2 : 1) {
+		const int wd = c ? *cwd : *lwd, n = c ? 2 : 1, infer = !(is_b && wd == 7) && rnd(g, 4) == 0;
+		for (int k = c; k < c + n; k++) {
+			int wk = wp_full_value(g, 1 << wd);
+			w[l][i][k] = (int16_t)(infer ? 1 << wd : wk > 127 ? 127 : wk);
+			o[l][i][k] = (int16_t)(infer ? 0 : wp_full_value(g, 0));
+		}
+	}
+	if (!is_b) return;
+	for (int c = 0; c < 3; c++) {
+		int mn = 127, mx = -128, top = (c ? *cwd : *lwd) == 7 ? 127 : 128;
+		for (int i = 0; i < n0; i++) { if (w[0][i][c] < mn) mn = w[0][i][c]; if (w[0][i][c] > mx) mx = w[0][i][c]; }
+		const int lo = -128 - mn > -128 ? -128 - mn : -128, hi = top - mx < 127 ? top - mx : 127;
+		for (int i = 0; i < 16; i++) {
+			int r = rnd(g, 4), v = r == 0 ? lo : r == 1 ? hi : w[1][i][c];
+			w[1][i][c] = (int16_t)(v < lo ? lo : v > hi ? hi : v);
+		}
+	}
+}
 
 /* returns 1 when the picture carried memory_management_control_operation 5 (frame_num and POC restart after it) */
 static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_pic_id) {
@@ -422,6 +490,7 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 			if (st == 1) bw_u(&w, 1, 0);
 			int wp = st == 0 ? g->wp_p : g->wp_b;
 			if (wp == 1) {
+				if (!w_ready && g->wp_full) { w_ready = 1; gen_wp_full(g, pp->type == 1, num_ref[0], &lwd, &cwd, w_tab, o_tab); }
 				if (!w_ready) { w_ready = 1;
 					lwd = rnd(g, pp->type == 1 ? 7 : 8); cwd = rnd(g, pp->type == 1 ? 7 : 8);   /* logWD 7 + inferred weight 128 is only legal for uni-prediction */
 					for (int l = 0; l < 2; l++) for (int i = 0; i < 16; i++) for (int c = 0; c < 3; c++) {
@@ -434,8 +503,14 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 				}
 				bw_ue(&w, lwd); bw_ue(&w, cwd);
 				for (int l = 0; l <= (st == 1); l++) for (int i = 0; i < num_ref[l]; i++) {
-					int lf = rnd(g, 4) != 0, cf = rnd(g, 4) != 0;
-					if (w_sent[l][i]) { lf = !(w_tab[l][i][0] == (1 << lwd) && o_tab[l][i][0] == 0); cf = 1; }
+					int lf, cf;
+					if (g->wp_full) {   /* the table holds the inferred values where a flag is to be 0 */
+						lf = !(w_tab[l][i][0] == (1 << lwd) && o_tab[l][i][0] == 0);
+						cf = !(w_tab[l][i][1] == (1 << cwd) && o_tab[l][i][1] == 0 && w_tab[l][i][2] == (1 << cwd) && o_tab[l][i][2] == 0);
+					} else {
+						lf = rnd(g, 4) != 0; cf = rnd(g, 4) != 0;
+						if (w_sent[l][i]) { lf = !(w_tab[l][i][0] == (1 << lwd) && o_tab[l][i][0] == 0); cf = 1; }
+					}
 					if (!lf) { w_tab[l][i][0] = (int16_t)(1 << lwd); o_tab[l][i][0] = 0; }
 					if (!cf) for (int c = 1; c < 3; c++) { w_tab[l][i][c] = (int16_t)(1 << cwd); o_tab[l][i][c] = 0; }
 					bw_u(&w, 1, lf); if (lf) { bw_se(&w, w_tab[l][i][0]); bw_se(&w, o_tab[l][i][0]); }
@@ -464,6 +539,7 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 		int cabac_init_idc = rnd(g, 3);
 		if (g->cabac && st != 2) bw_ue(&w, cabac_init_idc);
 		int slice_qp = g->qp0 + rnd(g, 7) - 3;
+		if (g->qp_walk) { int r = rnd(g, 4); slice_qp = r == 0 ? 0 : r == 1 ? 51 : rnd(g, 52); }
 		if (slice_qp < 0) slice_qp = 0;
 		if (slice_qp > 51) slice_qp = 51;
 		int pic_init_qp = g->qp0;
@@ -568,6 +644,13 @@ int main(int argc, char **argv) {
 	g->mixed = argf(argc, argv, "--mixed-slices"); g->ps_update = argf(argc, argv, "--ps-update");
 	g->dpb_mode = argf(argc, argv, "--dpb"); g->mmco5 = argf(argc, argv, "--mmco5"); g->poc_type = argi(argc, argv, "--poc-type", 0);
 	g->log2_max_frame_num = g->dpb_mode ? 4 : 8; g->log2_max_poc_lsb = 10;
+	for (int i = 1; i + 1 < argc; i++) {
+		if (!strcmp(argv[i], "--wp-range")) g->wp_full = !strcmp(argv[i + 1], "full");
+		if (!strcmp(argv[i], "--levels")) g->levels_big = !strcmp(argv[i + 1], "big");
+		if (!strcmp(argv[i], "--cqp-offset")) g->cqp_fixed = sscanf(argv[i + 1], "%d,%d", &g->cqp[0], &g->cqp[1]) == 2;
+	}
+	g->qp_walk = argf(argc, argv, "--qp-walk"); g->pcm_extreme = argf(argc, argv, "--pcm-extreme");
+	if (g->cqp_fixed && (g->cqp[0] < -12 || g->cqp[0] > 12 || g->cqp[1] < -12 || g->cqp[1] > 12)) { fprintf(stderr, "gen264: --cqp-offset takes two offsets in -12..12\n"); return 2; }
 	if ((g->dpb_mode && g->gop == 0) || (g->poc_type && g->gop != 1)) { fprintf(stderr, "gen264: --dpb needs --gop IP or IPB, --poc-type needs --gop IP\n"); return 2; }
 	if (g->slices > g->H) g->slices = g->H;
 	if (g->refs < 1) g->refs = 1;
