@@ -40,6 +40,9 @@ class Edge264Packed(ctypes.Structure):
                 ("on_device", ctypes.c_int32)]
 
 
+SKIP_NONE, SKIP_NONREF, SKIP_NONKEY = 0, 1, 2   # include/edge264_skip.h
+
+
 _loaded = {}
 
 
@@ -70,6 +73,8 @@ def bind(path):
     if hasattr(lib, "edge264_get_packed"):     # the extension of include/edge264_packed.h
         lib.edge264_enable_packed.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
         lib.edge264_get_packed.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264Packed)]
+    if hasattr(lib, "edge264_set_skip"):       # the extension of include/edge264_skip.h
+        lib.edge264_set_skip.argtypes = [ctypes.c_void_p, ctypes.c_int]
     _loaded[path] = lib
     return lib
 
@@ -148,12 +153,12 @@ def frame_packed(lib, dec, f):
     return out
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None):
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
     carries the frame's motion export (frame_motion); with packed=(format, log2_scale) it ends with the frame's packed
-    output (frame_packed)."""
+    output (frame_packed); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip)."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -174,6 +179,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             d = ctypes.c_void_p(dec)
             lib.edge264_free(ctypes.byref(d))
             raise RuntimeError("edge264_enable_packed: %s" % errno.errorcode.get(r, r))
+    if skip != SKIP_NONE:
+        r = lib.edge264_set_skip(dec, skip) if hasattr(lib, "edge264_set_skip") else errno.ENOTSUP
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_set_skip: %s" % errno.errorcode.get(r, r))
     nal = base + 3 + (1 if data[2] == 0 else 0)
     frames, codes, f = [], [], Edge264Frame()
     drained = False

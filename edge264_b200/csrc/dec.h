@@ -92,6 +92,7 @@ typedef struct Pic {
 	                           * poc/poc_top for output and later pictures only (8.2.1; reference headers.c:46-49, 673-680) */
 	int32_t uid;              /* unique id of the picture = FrameId */
 	int nonexisting;
+	int unfilled;             /* a skipped reference picture whose slot has not been filled yet (edge264_skip.h) */
 	E264MbRec *recs;          /* pinned host records of this picture (kept: co-located info for B direct) */
 	int32_t slot_uid[E264_MAX_SLOTS];   /* uid held by every slot when this picture was decoded */
 	int host_buf;             /* host mirror receiving the pixels; dropped (-1) once submitted AND queued for output */
@@ -205,6 +206,8 @@ struct Edge264Decoder {
 	Pic pics[E264_MAX_SLOTS];
 	int cur;                           /* slot of the picture being decoded, -1 none */
 	int cur_idr, cur_nal_ref_idc;
+	int cur_skip;                      /* the current picture is skipped: its headers run, its slice data is dropped */
+	int skip_mode;                     /* edge264_set_skip: applied to each picture at its first slice */
 	int prev_ref_frame_num, prev_ref_poc;   /* frame_num and POC of the previous reference picture (8.2.1) */
 	int q_prev_ref_frame_num, q_cur_frame_num;   /* reference-style absolute frame numbers, only used to number FrameIds like it */
 	int32_t next_uid;

@@ -17,6 +17,7 @@
 #include "h264_tables.h"
 #include "../../include/edge264_motion.h"
 #include "../../include/edge264_packed.h"
+#include "../../include/edge264_skip.h"
 
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
@@ -437,13 +438,15 @@ static int finish_picture(Edge264Decoder *d) {
 	if (d->cur < 0) return 0;
 	Pic *p = &d->pics[d->cur];
 	int ret = 0;
-	pthread_mutex_lock(&d->lock);
-	d->pb->conceal_ref = conceal_reference(d);
-	d->pb->closed = 1;
-	pthread_cond_broadcast(&d->work_cv);
-	if (!d->n_threads) ret = build_work(d, d->pb);
-	pthread_mutex_unlock(&d->lock);
-	d->pb = NULL;
+	if (d->pb) {   /* a skipped picture has no build */
+		pthread_mutex_lock(&d->lock);
+		d->pb->conceal_ref = conceal_reference(d);
+		d->pb->closed = 1;
+		pthread_cond_broadcast(&d->work_cv);
+		if (!d->n_threads) ret = build_work(d, d->pb);
+		pthread_mutex_unlock(&d->lock);
+		d->pb = NULL;
+	}
 	if (p->host_buf >= 0 && !p->needed_for_output) p->host_buf = -1;   /* already in the output queue */
 	apply_marking(d);
 	int c = d->cur;
@@ -492,12 +495,13 @@ static void slice_enqueue(Edge264Decoder *d, PicBuild *pb, SliceJob *job, int co
 	pthread_cond_broadcast(&d->work_cv);
 	pthread_mutex_unlock(&d->lock);
 }
-/* wait until every picture has been parsed and handed to the backend (flush, end of stream, format change) */
-static void threads_drain(Edge264Decoder *d) {
+/* wait until every picture but `except` (NULL: every picture) has been parsed and handed to the backend (flush, end of
+ * stream, format change, a fill of a frame slot) */
+static void threads_drain(Edge264Decoder *d, const PicBuild *except) {
 	pthread_mutex_lock(&d->lock);
 	for (;;) {
 		int busy = 0;
-		for (int i = 0; i < d->n_builds; i++) busy |= d->builds[i].in_use;
+		for (int i = 0; i < d->n_builds; i++) busy |= d->builds[i].in_use && &d->builds[i] != except;
 		if (!busy) break;
 		/* not reached without workers: the picture under construction, if any, was closed before, which submitted it */
 		pthread_cond_wait(&d->done_cv, &d->lock);
@@ -577,7 +581,7 @@ static void *worker_main(void *arg) {
 	return NULL;
 }
 static void threads_stop(Edge264Decoder *d) {
-	threads_drain(d);
+	threads_drain(d, NULL);
 	pthread_mutex_lock(&d->lock);
 	d->stop = 1;
 	pthread_cond_broadcast(&d->work_cv); pthread_cond_broadcast(&d->done_cv);
@@ -639,7 +643,7 @@ static void apply_marking(Edge264Decoder *d) {
 /* ------------------------------------------------------------------------------------------ */
 static int bump_all(Edge264Decoder *d) {
 	if (d->cur >= 0) finish_picture(d);
-	threads_drain(d);
+	threads_drain(d, NULL);
 	while (bump_frame(d, -1));
 	if (d->outq_n) return ENOBUFS;
 	/* frames the application still holds (borrowed, or handed out until the next decode_NAL) keep their buffers: a
@@ -912,7 +916,7 @@ static int fill_frame_num_gap(Edge264Decoder *d, int frame_num_abs) {
 		for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && d->pics[i].ref == 1 && (old < 0 || d->pics[i].frame_num < d->pics[old].frame_num)) old = i;
 		d->pics[old].ref = 0; slot_release_if_unused(d, old);
 	}
-	if (gap_frames > 0) threads_drain(d);   /* the fills below go straight to the device: every earlier picture must be on its way first */
+	if (gap_frames > 0) threads_drain(d, NULL);   /* the fills below go straight to the device: every earlier picture must be on its way first */
 	for (int fn = frame_num_abs - gap_frames; fn < frame_num_abs; fn++) {
 		int sl = find_free_slot(d);
 		while (sl < 0 && bump_frame(d, -1)) sl = find_free_slot(d);
@@ -950,9 +954,35 @@ static void number_frame_id(Edge264Decoder *d, int frame_num, int gap_frames) {
 	d->q_cur_frame_num = qfn;
 }
 
-/* first slice of a picture: frame number, POC, FrameId, host buffer, slot, build and staging, bumping; sets d->cur, d->pb */
+/* the data side of a decoded picture d->cur in `slot`: its host buffer, build and staging; sets d->pb */
+static int start_build(Edge264Decoder *d, int slot, int hbuf) {
+	Pic *cp = &d->pics[slot];
+	d->hb[hbuf].state = 1; d->hb[hbuf].frame_id = cp->uid; d->hb[hbuf].borrowed = 0; d->hb[hbuf].submitted = 0; d->hb[hbuf].err_pic = 0;
+	PicBuild *pb = build_acquire(d, slot);     /* may wait for a worker to finish a picture */
+	E264Staging stg; memset(&stg, 0, sizeof(stg));
+	int ar;
+	{ PROF_BEGIN; pthread_mutex_lock(&d->be_lock); ar = d->be->acquire_staging(d->be_ctx, slot, &stg); pthread_mutex_unlock(&d->be_lock); PROF_END(1); }
+	if (ar) {   /* give the build back as if it had never been taken (no later picture exists yet) */
+		pthread_mutex_lock(&d->lock); d->next_seq--; d->slot_users[slot]--; d->slot_build[slot] = NULL; pb->in_use = 0; pthread_mutex_unlock(&d->lock);
+		cp->in_use = 0; d->cur = -1; d->hb[hbuf].state = 0;
+		return ENOMEM;
+	}
+	cp->recs = stg.recs;
+	pb->recs = stg.recs; pb->coefs = stg.coefs; pb->slices = stg.slices; pb->intra_list = stg.intra_list; pb->staging = stg.handle;
+	pb->coef_cap = stg.coef_capacity; pb->n_coefs = 0; pb->n_slices = 0; pb->mbs_done = 0; pb->n_intra = 0; pb->any_deblock = 0;
+	pb->slot = slot; pb->host_buf = hbuf; pb->conceal_ref = -1; pb->slice_counter = 0;
+	memcpy(pb->slot_ids, cp->slot_uid, sizeof(pb->slot_ids));   /* slots may hold other pictures by the time this one is submitted */
+	{ PROF_BEGIN; memset(pb->mbi, 0, (size_t)d->w_mbs * d->h_mbs * sizeof(MbInfo)); PROF_END(4); }
+	/* records need no clearing: every macroblock of a complete picture rewrites its own (sx_one_mb) */
+	d->pb = pb;
+	return 0;
+}
+
+/* first slice of a picture: frame number, POC, FrameId, slot, the data side (start_build) unless the picture is skipped,
+ * bumping; sets d->cur, d->cur_skip */
 static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int nal_ref_idc) {
 	const SPS *s = &d->sps;
+	int ret;
 	if (d->outq_n > 16) {
 		/* the frame the application is told to fetch may still be with a parser: wait for it here, not in a polling
 		 * loop (without workers every queued frame has been submitted, so this does not wait) */
@@ -961,8 +991,10 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 		pthread_mutex_unlock(&d->lock);
 		return ENOBUFS;
 	}
-	int hbuf = hostbuf_acquire(d);
-	if (hbuf < 0) return ENOBUFS;
+	/* edge264_skip.h: decided once, at the picture's first slice */
+	const int skip = d->skip_mode == EDGE264_SKIP_NONREF ? !nal_ref_idc : d->skip_mode == EDGE264_SKIP_NONKEY ? !idr && h->slice_type != 2 : 0;
+	int hbuf = -1;
+	if (!skip && (hbuf = hostbuf_acquire(d)) < 0) return ENOBUFS;
 	/* absolute (unwrapped) frame numbers like the reference (headers.c:1059) */
 	int prev = d->prev_ref_frame_num;
 	int frame_num_abs = idr ? 0 : prev + 1 + ((h->frame_num - prev - 1) & ((1 << s->log2_max_frame_num) - 1));
@@ -981,27 +1013,12 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 	memset(cp, 0, sizeof(*cp));
 	number_frame_id(d, idr ? 0 : h->frame_num, gap_frames);
 	cp->in_use = 1; cp->frame_num = frame_num_abs; cp->poc = cp->poc_dec = poc; cp->poc_top = cp->poc_top_dec = poc_top; cp->uid = d->next_uid++; cp->host_buf = hbuf;
-	d->hb[hbuf].state = 1; d->hb[hbuf].frame_id = cp->uid; d->hb[hbuf].borrowed = 0; d->hb[hbuf].submitted = 0; d->hb[hbuf].err_pic = 0;
-	d->cur = slot; d->cur_idr = idr; d->cur_nal_ref_idc = nal_ref_idc;
+	d->cur = slot; d->cur_idr = idr; d->cur_nal_ref_idc = nal_ref_idc; d->cur_skip = skip;
 	d->first_sh = *h;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = d->pics[i].in_use ? d->pics[i].uid : -1;
-	PicBuild *pb = build_acquire(d, slot);     /* may wait for a worker to finish a picture */
-	E264Staging stg; memset(&stg, 0, sizeof(stg));
-	int ar;
-	{ PROF_BEGIN; pthread_mutex_lock(&d->be_lock); ar = d->be->acquire_staging(d->be_ctx, slot, &stg); pthread_mutex_unlock(&d->be_lock); PROF_END(1); }
-	if (ar) {   /* give the build back as if it had never been taken (no later picture exists yet) */
-		pthread_mutex_lock(&d->lock); d->next_seq--; d->slot_users[slot]--; d->slot_build[slot] = NULL; pb->in_use = 0; pthread_mutex_unlock(&d->lock);
-		cp->in_use = 0; d->cur = -1; d->hb[hbuf].state = 0;
-		return ENOMEM;
-	}
-	cp->recs = stg.recs;
-	pb->recs = stg.recs; pb->coefs = stg.coefs; pb->slices = stg.slices; pb->intra_list = stg.intra_list; pb->staging = stg.handle;
-	pb->coef_cap = stg.coef_capacity; pb->n_coefs = 0; pb->n_slices = 0; pb->mbs_done = 0; pb->n_intra = 0; pb->any_deblock = 0;
-	pb->slot = slot; pb->host_buf = hbuf; pb->conceal_ref = -1; pb->slice_counter = 0;
-	memcpy(pb->slot_ids, cp->slot_uid, sizeof(pb->slot_ids));   /* slots may hold other pictures by the time this one is submitted */
-	{ PROF_BEGIN; memset(pb->mbi, 0, (size_t)d->w_mbs * d->h_mbs * sizeof(MbInfo)); PROF_END(4); }
-	/* records need no clearing: every macroblock of a complete picture rewrites its own (sx_one_mb) */
-	d->pb = pb;
+	if (skip) {   /* no build, no staging: a non-existing frame whose slot is filled if a decoded picture ever predicts from it */
+		cp->nonexisting = 1; cp->unfilled = nal_ref_idc != 0;
+	} else if ((ret = start_build(d, slot, hbuf))) return ret;
 
 	/* IDR / MMCO5: every earlier picture leaves in output order first (reference headers.c:632, 680) */
 	int has_mmco5 = 0;
@@ -1017,10 +1034,10 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 		for (int i = 0; i < d->n_slots; i++) if (i != slot && d->pics[i].in_use && d->pics[i].needed_for_output && d->pics[i].poc_top < cp->poc_top) max_bump++;
 	}
 	while (dpb_fullness(d) >= s->max_dec_frame_buffering && max_bump--) bump_frame(d, slot);
-	cp->needed_for_output = 1;
+	cp->needed_for_output = 1;   /* a skipped picture too: it leaves by bumping as in a full decode, without a buffer to queue */
 	if (max_bump < 0) {   /* nothing may precede it: straight to the output queue (it is returned once decoded) */
 		cp->needed_for_output = 0;
-		d->hb[hbuf].state = 2; d->outq[d->outq_n++] = hbuf;
+		if (!skip) { d->hb[hbuf].state = 2; d->outq[d->outq_n++] = hbuf; }
 	} else if (waiting_for_output(d) > s->max_num_reorder_frames) bump_frame(d, -1);
 	/* POC bookkeeping for the next picture (8.2.1.1) */
 	if (nal_ref_idc) { d->prev_ref_poc = has_mmco5 ? cp->poc_top : poc_top; }
@@ -1044,6 +1061,17 @@ static void implicit_weights(const SliceCtx *c, E264SliceRec *sr) {
 		}
 		sr->implicit_w1[i0][i1] = (int16_t)w1;
 	}
+}
+
+/* A skipped reference picture named by a decoded picture's reference list gets its samples now, like the frames of a
+ * frame_num gap (edge264_skip.h): a constant, and an error map of 100 that the taint carries into the predicting picture.
+ * The fill goes straight to the device, after every earlier picture and before the current one. */
+static void fill_skipped(Edge264Decoder *d, int slot) {
+	if (!d->pics[slot].unfilled) return;
+	d->pics[slot].unfilled = 0;
+	threads_drain(d, d->pb);
+	if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, slot, 0, 0); pthread_mutex_unlock(&d->be_lock); }
+	d->taint |= 1u << slot;
 }
 
 /* slice record (deblocking, weights, scaling lists) and parsing context (reference lists, co-located slot in *col_slot) */
@@ -1076,6 +1104,7 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 	if (h->slice_type < 2) {
 		int lists[2][32], nl[2];
 		build_ref_lists(d, h, lists, nl);
+		for (int l = 0; l <= (h->slice_type == 1); l++) for (int i = 0; i < h->num_ref[l]; i++) if (lists[l][i] >= 0) fill_skipped(d, lists[l][i]);
 		for (int l = 0; l <= (h->slice_type == 1); l++) {
 			/* a missing entry (damaged or non-conforming stream) is predicted from a defined picture other than the one
 			 * being decoded: the list's first present entry, else the picture concealment copies from.  It keeps
@@ -1130,6 +1159,7 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, B
 		if (newpic) { ret = finish_picture(d); if (ret) return ret; }
 	}
 	if (d->cur < 0 && (ret = start_picture(d, h, nal_unit_type == 5, nal_ref_idc))) return ret;
+	if (d->cur_skip) return h->first_mb >= d->w_mbs * d->h_mbs ? EBADMSG : 0;   /* its slice data is never parsed */
 	int col_slot;
 	if ((ret = setup_slice(d, p, h, b, *jobp, &col_slot))) return ret;
 	PicBuild *pb = d->pb;
@@ -1176,7 +1206,7 @@ Edge264Decoder *edge264_alloc(int n_threads, Edge264LogCb log_cb, void *log_arg,
 void edge264_flush(Edge264Decoder *d) {
 	if (!d) return;
 	finish_picture(d);
-	threads_drain(d);
+	threads_drain(d, NULL);
 	/* drop every picture and the sequence state, keep parameter sets (reference edge264.c:261-270 clears them too) */
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { d->pics[i].in_use = 0; d->pics[i].host_buf = -1; }
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state != 3 || !d->hb[i].borrowed) d->hb[i].state = 0;
@@ -1351,5 +1381,14 @@ int edge264_get_packed(Edge264Decoder *d, const Edge264Frame *frame, Edge264Pack
 	out->width = l.width; out->height = l.height; out->width_C = l.width_C; out->height_C = l.height_C;
 	out->format = hb->pk.format; out->log2_scale = hb->pk.log2_scale;
 	out->on_device = hb->packed_dev;
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* skipped pictures (include/edge264_skip.h)                                                    */
+/* ------------------------------------------------------------------------------------------ */
+int edge264_set_skip(Edge264Decoder *d, int mode) {
+	if (!d || mode < EDGE264_SKIP_NONE || mode > EDGE264_SKIP_NONKEY) return EINVAL;
+	d->skip_mode = mode;   /* read by start_picture only: the current picture keeps its decision */
 	return 0;
 }

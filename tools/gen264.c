@@ -17,6 +17,9 @@
  *          [--nonref-p]                     (with --gop IP: some P pictures are not used for reference)
  *          [--extra-nals]                   (access unit delimiters, SEI and filler data NAL units between pictures)
  *          [--bref]                         (with --gop IPB: the first B picture of each pair is a reference picture)
+ *          [--i-period N]                   (with --gop IP / IPB: a non-IDR I picture in place of the next P anchor once
+ *                                           N pictures have been coded since the last I or IDR picture; the pictures
+ *                                           after it may still predict from pictures before it: open GOP)
  *          [--mixed-slices]                 (slices of one picture take different slice types)
  *          [--ps-update]                    (picture parameter sets re-sent with new chroma QP offsets, and the unchanged
  *                                            sequence parameter set repeated, between pictures)
@@ -55,6 +58,7 @@ typedef struct GenState {
 	int log2_max_frame_num, log2_max_poc_lsb;
 	int drift[2];           /* per-picture global motion */
 	int cur_is_b;
+	int i_period;
 	int direct4x4, nonref_p, extra_nals, bref, crop_left, crop_right, crop_top, mixed, ps_update, dpb_mode, mmco5, poc_type, max_long_idx_plus1, stat_rplm, stat_mmco[7], stat_idr_long;   /* --dpb: list modification + memory-management stress on I P P P streams; --poc-type 0|1|2 */
 	int wp_full, qp_walk, cqp_fixed, cqp[2], levels_big, pcm_extreme;   /* the standard's limits (file header) */
 } GenState;
@@ -641,6 +645,7 @@ int main(int argc, char **argv) {
 	g->crop_left = argi(argc, argv, "--crop-left", 0); g->crop_right = argi(argc, argv, "--crop-right", 0); g->crop_top = argi(argc, argv, "--crop-top", 0);
 	g->direct4x4 = argf(argc, argv, "--direct4x4"); g->nonref_p = argf(argc, argv, "--nonref-p"); g->extra_nals = argf(argc, argv, "--extra-nals");
 	g->bref = argf(argc, argv, "--bref");
+	g->i_period = argi(argc, argv, "--i-period", 0);
 	g->mixed = argf(argc, argv, "--mixed-slices"); g->ps_update = argf(argc, argv, "--ps-update");
 	g->dpb_mode = argf(argc, argv, "--dpb"); g->mmco5 = argf(argc, argv, "--mmco5"); g->poc_type = argi(argc, argv, "--poc-type", 0);
 	g->log2_max_frame_num = g->dpb_mode ? 4 : 8; g->log2_max_poc_lsb = 10;
@@ -660,7 +665,7 @@ int main(int argc, char **argv) {
 	g->mbi = (MbInfo *)calloc((size_t)nmb, sizeof(MbInfo));
 	g->pool = (int16_t *)calloc((size_t)nmb * 408 + 1024, sizeof(int16_t));
 	ByteBuf out = {0, 0, 0};
-	int frame_num = 0, idr_id = 0, disp = 0, since_idr = 0;
+	int frame_num = 0, idr_id = 0, disp = 0, since_idr = 0, since_i = 0;
 	/* coding order.  gop 0: IDR every picture; gop 1: IDR P P P ...; gop 2: IDR P B B P B B ... (B not referenced) */
 	for (int k = 0; k < g->frames;) {
 		int need_idr = k == 0 || since_idr >= g->idr_period;
@@ -670,7 +675,7 @@ int main(int argc, char **argv) {
 			PicPlan p = {2, 1, 1, 0, 0};
 			frame_num = 0; disp = 0; since_idr = 0;
 			encode_picture(g, &out, &p, idr_id++ & 0xffff);
-			frame_num = 1; disp = 1; since_idr = 1; k++;
+			frame_num = 1; disp = 1; since_idr = 1; since_i = 1; k++;
 			continue;
 		}
 		if (g->ps_update && rnd(g, 4) == 0) { if (rnd(g, 3) == 0) write_sps(g, &out); for (int id = 0; id < 3; id++) write_pps(g, &out, id, g->qp0); }
@@ -679,19 +684,21 @@ int main(int argc, char **argv) {
 			if (rnd(g, 3) == 0) { uint8_t sei[40]; int n = 2 + rnd(g, 30); sei[0] = 5; sei[1] = (uint8_t)n; for (int i = 0; i < n; i++) sei[2 + i] = (uint8_t)rnd(g, 256); sei[2 + n] = 0x80; e264_emit_nal(&out, 0, 6, sei, 3 + n); }
 			if (rnd(g, 4) == 0) { uint8_t fil[24]; int n = 1 + rnd(g, 20); for (int i = 0; i < n; i++) fil[i] = 0xff; fil[n] = 0x80; e264_emit_nal(&out, 0, 12, fil, n + 1); }
 		}
+		const int i_pic = g->i_period > 0 && since_i >= g->i_period;   /* --i-period: this anchor is a non-IDR I picture */
+		if (i_pic) since_i = 0;
 		if (g->gop == 1) {
-			const int is_ref = !(g->nonref_p && g->poc_type == 0 && !g->dpb_mode && rnd(g, 3) == 0);
-			PicPlan p = {0, 0, is_ref, frame_num, disp * 2};
+			const int is_ref = i_pic || !(g->nonref_p && g->poc_type == 0 && !g->dpb_mode && rnd(g, 3) == 0);
+			PicPlan p = {i_pic ? 2 : 0, 0, is_ref, frame_num, disp * 2};
 			if (encode_picture(g, &out, &p, 0)) { frame_num = 0; disp = 0; }
 			if (is_ref) frame_num++;
-			disp++; since_idr++; k++;
+			disp++; since_idr++; since_i++; k++;
 			continue;
 		}
 		/* IPB: next anchor P at display disp+2 (or fewer if the sequence ends), then the B pictures before it */
 		int nb = 2;
 		if (k + 1 + nb > g->frames) nb = g->frames - k - 1;
 		if (since_idr + 1 + nb > g->idr_period) nb = g->idr_period - since_idr - 1 < 0 ? 0 : g->idr_period - since_idr - 1;
-		PicPlan p = {0, 0, 1, frame_num, (disp + nb) * 2};
+		PicPlan p = {i_pic ? 2 : 0, 0, 1, frame_num, (disp + nb) * 2};
 		encode_picture(g, &out, &p, 0);
 		frame_num++; k++;
 		for (int b = 0; b < nb; b++) {
@@ -700,7 +707,7 @@ int main(int argc, char **argv) {
 			const int can_ref = used < g->refs || nshort > 0;   /* the sliding window needs a short-term picture to drop */
 			PicPlan q = {1, 0, g->bref && b == 0 && nb == 2 && can_ref, frame_num, (disp + b) * 2}; encode_picture(g, &out, &q, 0); if (q.is_ref) frame_num++; k++;
 		}
-		disp += nb + 1; since_idr += nb + 1;
+		disp += nb + 1; since_idr += nb + 1; since_i += nb + 1;
 	}
 	FILE *f = fopen(outp, "wb");
 	if (!f) { perror(outp); return 2; }
