@@ -693,6 +693,7 @@ extern "C" uint64_t e264b_slot_hash(E264bDevice *c, int slot) {
  * width x height samples without stride padding (Y, then Cb, then Cr) to out + k * e264b_picture_bytes(c).  Before that
  * it reads the slots as the previous replay left them: every slot's last writer must come out identical again.
  * Returns 0, -1 on a CUDA error, -2 when a picture differs from what the previous replay left in its slot. */
+extern "C" int e264b_slot_count(E264bDevice *c) { return c->n_slots; }
 extern "C" long long e264b_picture_bytes(E264bDevice *c) { return (long long)c->g.width_mbs * 16 * c->g.height_mbs * 16 * 3 / 2; }
 static int copy_picture(E264bDevice *c, int slot, uint8_t *o) {
 	const size_t w = (size_t)c->g.width_mbs * 16, h = (size_t)c->g.height_mbs * 16;

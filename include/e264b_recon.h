@@ -70,6 +70,7 @@ typedef struct E264bReplayStats {
 } E264bReplayStats;
 int      e264b_replay(E264bDevice **devs, int n, int reps, int threads, E264bReplayStats *stats);
 uint64_t e264b_slot_hash(E264bDevice *dev, int slot);
+int      e264b_slot_count(E264bDevice *dev);                  /* frame slots of the geometry last configured */
 long long e264b_picture_bytes(E264bDevice *dev);              /* width x height x 3/2 */
 int      e264b_replay_frames(E264bDevice *dev, uint8_t *out);  /* every kept picture once more, in decode order, into out */
 /* known-answer support (tests): one block through the device's intra predictors (fn 0-3) or luma interpolation (fn 4) */

@@ -2,11 +2,21 @@
  * device (libedge264_b200.so's e264b_* entry points) and through the CPU restatement (oracle/port_recon.c); every frame
  * must come out byte for byte the same.  Every picture keeps the record contract (oracle/record_check.c) before either
  * side sees it.  tests/test_record_fuzz.py builds and runs it.
- *   record_fuzz [--cpu-only] [--lib libedge264_b200.so] [--seeds A-B] [--pictures N] [--geom WxH]
+ *   record_fuzz [--cpu-only] [--lib libedge264_b200.so] [--seeds A-B] [--pictures N] [--geom WxH] [--contexts M] [--inflight K]
  * --cpu-only generates, checks and reconstructs on the CPU restatement only.  At the end it prints one line per coverage
- * counter ("cov NAME VALUE"), counted from the generated inputs and, for saturation and wrap-around, in the port. */
+ * counter ("cov NAME VALUE"), counted from the generated inputs and, for saturation and wrap-around, in the port.
+ * --contexts M --inflight K (default 1 and 1: one picture at a time, compared before the next is drawn) runs M device
+ * contexts on M host threads, each taking every M-th seed with its own geometry, slot count and number of staging areas
+ * (often fewer than K).  A context draws K pictures, reconstructing each on the port at once and keeping the port's
+ * frame, then submits the K back to back, each with its own output buffer, and only then waits for them and compares
+ * them in order.  References stay random among the other slots, biased towards the slot of the picture drawn just
+ * before, so that pictures read slots that pictures in flight still write and overwrite slots they still read.  Extra
+ * counters: inflight_max, contexts, ref_slot_in_flight, dst_slot_read_in_flight, and staging_wrapped (pictures submitted
+ * while every staging area of the context was in use, so that e264b_acquire_staging had to wait), after one line of
+ * pictures per context. */
 #define _GNU_SOURCE
 #include <dlfcn.h>
+#include <pthread.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -20,6 +30,9 @@
 void port_recon_picture(uint8_t *frames, const E264PicDesc *pd, const E264MbRec *recs, const int16_t *coefs, const E264SliceRec *slices);
 int port_boundary_strength(const E264MbRec *p, int bp, const E264MbRec *q, int bq, int mb_edge);
 extern long port_cov_residual[6], port_cov_wp_bi_sat16;
+/* the port counts its saturation and wrap-around events (and its E264_COVERAGE limits) in process-wide counters: the
+ * contexts' host threads reconstruct on it one at a time */
+static pthread_mutex_t port_mu = PTHREAD_MUTEX_INITIALIZER;
 
 /* ---- the device, through the product library's C ABI (include/e264b_recon.h) ---- */
 static struct {
@@ -45,8 +58,9 @@ static void load_device(const char *lib) {
 #undef SYM
 }
 
-/* ---- random numbers ---- */
-static uint64_t rng;
+/* ---- random numbers (the generator's state is per host thread: each context draws its own pictures; the coverage
+ * counters below too, summed when the thread ends) ---- */
+static _Thread_local uint64_t rng;
 static uint32_t r32(void) { rng ^= rng >> 12; rng ^= rng << 25; rng ^= rng >> 27; return (uint32_t)((rng * 0x2545F4914F6CDD1Dull) >> 32); }
 static int rnd(int n) { return n > 0 ? (int)(r32() % (unsigned)n) : 0; }
 static int pct(int p) { return rnd(100) < p; }
@@ -60,21 +74,32 @@ enum {
 	C_BS,   /* 30 entries: [left, top, internal][t4x4, t8x8][bS 0..4] */
 	C_FOFF_M12 = C_BS + 30, C_FOFF_P12, C_IDC0, C_IDC1, C_IDC2, C_SLICES64,
 	C_INTRA_COMBOS, C_IPCM, C_CONCEAL_INTER, C_CONCEAL_INTRA,
-	C_FRAC_0, C_FRAC_1, C_FRAC_BELOW, C_FRAC_AT, C_FRAC_ABOVE, C_FRAC_ALL, C_WP_LWD7_BRIGHT, C_PICTURES, C_N
+	C_FRAC_0, C_FRAC_1, C_FRAC_BELOW, C_FRAC_AT, C_FRAC_ABOVE, C_FRAC_ALL, C_WP_LWD7_BRIGHT, C_PICTURES,
+	C_INFLIGHT_MAX, C_REF_IN_FLIGHT, C_DST_READ_IN_FLIGHT, C_STAGING_WRAPPED, C_CONTEXTS, C_N   /* counted with pictures in flight */
 };
-static long cov[C_N];
-static uint64_t qp_seen[3];
-static uint8_t intra_seen[3 + 1][9][16];   /* kind (I4x4, I8x8, I16x16, chroma) x mode x unavailability */
+static _Thread_local long cov[C_N];
+static _Thread_local uint64_t qp_seen[3];
+static _Thread_local uint8_t intra_seen[3 + 1][9][16];   /* kind (I4x4, I8x8, I16x16, chroma) x mode x unavailability */
 static const char *bs_name(int i) {
 	static char b[40]; snprintf(b, sizeof(b), "bs_%s_%s_%d", (i / 10) == 0 ? "left" : (i / 10) == 1 ? "top" : "internal", (i / 5) & 1 ? "t8x8" : "t4x4", i % 5); return b;
 }
 
 /* ---- geometry and frames ---- */
+#define FUZZ_NSTAGE 8   /* staging areas e264b_configure allocates at most (NSTAGE of recon.cu) */
+typedef struct {        /* a picture drawn and reconstructed on the port, not yet compared with the device */
+	int pic, dst; uint32_t reads;               /* reads: bit s = some block predicts from slot s */
+	E264PicDesc pd; uint64_t ticket;
+	uint8_t *host_out, *port;                   /* the device's frame (e264b_host_alloc) and the port's frame of the same slot */
+	E264MbRec *recs; int16_t *coefs; E264SliceRec *slices; uint32_t *intra_list;   /* its records */
+} Pending;
 typedef struct {
 	E264PicDesc g; int n_slots, nmb;
 	uint8_t *port_frames, *port_alloc;     /* the port's frame slots */
 	E264MbRec *recs; int16_t *coefs; uint32_t coef_cap; E264SliceRec *slices; uint32_t *intra_list;   /* one picture being built */
-	void *dev; uint8_t *host_out;
+	void *dev;
+	int inflight, n_stage;                 /* pictures submitted ahead at most; staging areas of the device context */
+	Pending *q; int q_head, n_out;         /* the pictures drawn and not yet compared, oldest first */
+	int prev_dst;                          /* slot of the picture drawn last (with pictures in flight) */
 } Ctx;
 
 static void geometry(Ctx *c, int W, int H, int n_slots) {
@@ -184,13 +209,30 @@ static void draw_mv(Ctx *c, int mbx, int mby, int b, int16_t mv[2], const int16_
 	}
 }
 
+/* a reference slot other than dst; with pictures in flight, often the slot of the picture submitted just before it */
+static int draw_ref(Ctx *c, int dst) {
+	if (c->inflight > 1 && c->prev_dst != dst && pct(25)) return c->prev_dst;
+	int ref = rnd(c->n_slots - 1);
+	return ref >= dst ? ref + 1 : ref;
+}
+
+/* the slot of the next picture; with pictures in flight, often one that a picture in flight predicts from */
+static int draw_dst(Ctx *c) {
+	if (c->inflight > 1 && c->n_out && pct(30)) {
+		uint32_t m = 0;
+		for (int k = 0; k < c->n_out; k++) m |= c->q[(c->q_head + k) % c->inflight].reads;
+		if (m) { int n = rnd(__builtin_popcount(m)); while (n--) m &= m - 1; return __builtin_ctz(m); }
+	}
+	return rnd(c->n_slots);
+}
+
 /* draw the records of one picture into c->recs / coefs / slices; returns n_coefs */
 static void draw_picture(Ctx *c, E264PicDesc *pd, int dst, int pcm_content) {
 	const int W = c->g.width_mbs, nmb = c->nmb;
 	*pd = c->g; pd->dst_slot = dst;
 	/* slices: contiguous runs in raster order */
 	int n_slices = pcm_content >= 0 ? 1 : pct(10) && nmb >= MAX_SLICES ? MAX_SLICES : 1 + rnd(nmb < 8 ? nmb : 8);
-	static int start[MAX_SLICES + 1];
+	static _Thread_local int start[MAX_SLICES + 1];
 	start[0] = 0;
 	for (int i = 1; i < n_slices; i++) start[i] = i;                 /* distinct cut points */
 	for (int i = 1; i < n_slices; i++) { int lo = start[i - 1] + 1, hi = nmb - (n_slices - i); start[i] = lo + rnd(hi - lo + 1); }
@@ -203,7 +245,7 @@ static void draw_picture(Ctx *c, E264PicDesc *pd, int dst, int pcm_content) {
 	if (pcm_content >= 0) n_want = nmb;
 	if (n_want < 0) n_want = 0;
 	if (n_want > nmb) n_want = nmb;
-	static uint8_t is_intra[1 << 16];
+	static _Thread_local uint8_t is_intra[1 << 16];
 	memset(is_intra, 0, (size_t)nmb);
 	for (int k = 0, left = n_want; k < nmb; k++) { if (rnd(nmb - k) < left) { is_intra[k] = 1; left--; } }
 	cov[C_FRAC_0] += n_want == 0; cov[C_FRAC_1] += n_want == 1; cov[C_FRAC_ALL] += n_want == nmb && nmb > 2;
@@ -229,7 +271,7 @@ static void draw_picture(Ctx *c, E264PicDesc *pd, int dst, int pcm_content) {
 			if (is_intra[a]) { r->kind = MBK_I16x16; r->i16_mode = IMODE(2, 11); r->chroma_mode = IMODE(0, 11); cov[C_CONCEAL_INTRA]++; }
 			else {
 				r->kind = MBK_INTER; r->flags = MBF_SKIP;
-				int ref = rnd(c->n_slots - 1); if (ref >= dst) ref++;
+				int ref = draw_ref(c, dst);
 				for (int i8 = 0; i8 < 4; i8++) { r->ref_idx[0][i8] = 0; r->ref_pic[0][i8] = (int8_t)ref; }
 				cov[C_CONCEAL_INTER]++;
 			}
@@ -261,7 +303,7 @@ static void draw_picture(Ctx *c, E264PicDesc *pd, int dst, int pcm_content) {
 						int use = 1 + rnd(3);
 						for (int l = 0; l < 2; l++) if (use >> l & 1) {
 							r->ref_idx[l][i8] = (int8_t)rnd(16);
-							int ref = rnd(c->n_slots - 1); if (ref >= dst) ref++;
+							int ref = draw_ref(c, dst);
 							if (l == 1 && use == 3 && pct(30)) ref = r->ref_pic[0][i8];   /* one picture in both lists */
 							r->ref_pic[l][i8] = (int8_t)ref;
 						}
@@ -365,20 +407,63 @@ static void count_picture(Ctx *c) {
 	}
 }
 
-static void dump_mb(Ctx *c, int a) {
-	const E264MbRec *r = c->recs + a;
-	fprintf(stderr, "  mb %d (%d,%d) kind %d flags %02x qp %d %d %d chroma %02x i16 %02x slice %d coded %08x coef_off %u\n  modes", a, a % c->g.width_mbs, a / c->g.width_mbs,
+static void dump_mb(const E264MbRec *recs, const E264SliceRec *slices, int W, int a) {
+	const E264MbRec *r = recs + a;
+	fprintf(stderr, "  mb %d (%d,%d) kind %d flags %02x qp %d %d %d chroma %02x i16 %02x slice %d coded %08x coef_off %u\n  modes", a, a % W, a / W,
 	        r->kind, r->flags, r->qp[0], r->qp[1], r->qp[2], r->chroma_mode, r->i16_mode, r->slice_idx, r->coded, r->coef_off);
 	for (int i = 0; i < 16; i++) fprintf(stderr, " %02x", r->modes[i]);
 	fprintf(stderr, "\n  ref_idx"); for (int i = 0; i < 8; i++) fprintf(stderr, " %d", ((const int8_t *)r->ref_idx)[i]);
 	fprintf(stderr, " ref_pic"); for (int i = 0; i < 8; i++) fprintf(stderr, " %d", ((const int8_t *)r->ref_pic)[i]);
 	for (int l = 0; l < 2; l++) { fprintf(stderr, "\n  mv%d", l); for (int i = 0; i < 16; i++) fprintf(stderr, " (%d,%d)", r->mv[l][i][0], r->mv[l][i][1]); }
-	const E264SliceRec *s = c->slices + r->slice_idx;
+	const E264SliceRec *s = slices + r->slice_idx;
 	fprintf(stderr, "\n  slice: offsets %d %d idc %d wp %d log2_wd %d %d scaling4x4[0][0] %d scaling8x8[0][0] %d\n", s->filter_offset_a, s->filter_offset_b, s->deblock_idc,
 	        s->wp_mode, s->luma_log2_wd, s->chroma_log2_wd, s->scaling4x4[0][0], s->scaling8x8[0][0]);
 }
 
-/* one picture through both sides; returns 0 when they agree */
+/* wait for the oldest picture in flight and compare it with the port's frame of the same picture; returns 0 when they agree */
+static int retire(Ctx *c, int cpu_only) {
+	Pending *p = c->q + c->q_head;
+	c->q_head = (c->q_head + 1) % c->inflight; c->n_out--;
+	if (cpu_only) return 0;
+	if (D.wait(c->dev, p->ticket)) { fprintf(stderr, "picture %d: wait failed\n", p->pic); return 1; }
+	const int W = c->g.width_mbs, H = c->g.height_mbs;
+	for (int pl = 0; pl < 3; pl++) {
+		int w = pl ? W * 8 : W * 16, h = pl ? H * 8 : H * 16, stride = pl ? c->g.stride_c : c->g.stride_y;
+		size_t base = pl == 0 ? 0 : (size_t)c->g.plane_y + (pl == 2 ? c->g.stride_c / 2 : 0);
+		for (int y = 0; y < h; y++) for (int x = 0; x < w; x++) {
+			size_t o = base + (size_t)y * stride + x;
+			if (p->host_out[o] == p->port[o]) continue;
+			int a = (y / (pl ? 8 : 16)) * W + x / (pl ? 8 : 16);
+			fprintf(stderr, "MISMATCH picture %d (slot %d, %dx%d macroblocks, %d intra) plane %d x %d y %d: device %d port %d\n", p->pic, p->dst, W, H, p->pd.n_intra, pl, x, y, p->host_out[o], p->port[o]);
+			dump_mb(p->recs, p->slices, W, a);
+			return 1;
+		}
+	}
+	return 0;
+}
+
+/* submit every picture drawn since the last comparison, back to back so that the device is still working on the earlier
+ * ones (the port is far slower than the device: a picture submitted on its own is finished before the next is drawn),
+ * then compare them in order; returns 0 while the device agrees with the port */
+static int flush(Ctx *c, int cpu_only) {
+	for (int k = 0; k < c->n_out && !cpu_only; k++) {
+		Pending *p = c->q + (c->q_head + k) % c->inflight;
+		E264Staging st;
+		if (D.acquire(c->dev, p->dst, &st)) { fprintf(stderr, "acquire_staging failed\n"); exit(3); }
+		memcpy(st.recs, p->recs, (size_t)c->nmb * sizeof(E264MbRec));
+		memcpy(st.coefs, p->coefs, (size_t)p->pd.n_coefs * 2);
+		memcpy(st.slices, p->slices, (size_t)p->pd.n_slices * sizeof(E264SliceRec));
+		memcpy(st.intra_list, p->intra_list, (size_t)p->pd.n_intra * 4);
+		p->pd.staging = st.handle;
+		if (D.submit(c->dev, &p->pd, p->host_out, &p->ticket)) { fprintf(stderr, "picture %d: submit failed\n", p->pic); exit(3); }
+	}
+	int bad = 0;
+	while (c->n_out && !bad) bad = retire(c, cpu_only);
+	return bad;
+}
+
+/* one picture: drawn and reconstructed on the port at once, in draw order; it goes to the device with the pictures drawn
+ * before it once c->inflight pictures are waiting.  Returns 0 while the device agrees with the port */
 static int run_picture(Ctx *c, int pic, int dst, int pcm_content, int cpu_only) {
 	E264PicDesc pd;
 	draw_picture(c, &pd, dst, pcm_content);
@@ -389,63 +474,68 @@ static int run_picture(Ctx *c, int pic, int dst, int pcm_content, int cpu_only) 
 	}
 	count_picture(c);
 	cov[C_PICTURES]++;
-	port_recon_picture(c->port_frames, &pd, c->recs, c->coefs, c->slices);
-	if (cpu_only) return 0;
-	E264Staging st;
-	if (D.acquire(c->dev, dst, &st)) { fprintf(stderr, "acquire_staging failed\n"); exit(3); }
-	memcpy(st.recs, c->recs, (size_t)c->nmb * sizeof(E264MbRec));
-	memcpy(st.coefs, c->coefs, (size_t)pd.n_coefs * 2);
-	memcpy(st.slices, c->slices, (size_t)pd.n_slices * sizeof(E264SliceRec));
-	memcpy(st.intra_list, c->intra_list, (size_t)pd.n_intra * 4);
-	pd.staging = st.handle;
-	uint64_t t;
-	if (D.submit(c->dev, &pd, c->host_out, &t) || D.wait(c->dev, t)) { fprintf(stderr, "picture %d: submit/wait failed\n", pic); return 1; }
-	if (D.error_flag(c->dev)) { fprintf(stderr, "picture %d: device error flag %d\n", pic, D.error_flag(c->dev)); return 1; }
-	const uint8_t *port = c->port_frames + (size_t)dst * c->g.frame_bytes;
-	const int W = c->g.width_mbs, H = c->g.height_mbs;
-	for (int pl = 0; pl < 3; pl++) {
-		int w = pl ? W * 8 : W * 16, h = pl ? H * 8 : H * 16, stride = pl ? c->g.stride_c : c->g.stride_y;
-		size_t base = pl == 0 ? 0 : (size_t)c->g.plane_y + (pl == 2 ? c->g.stride_c / 2 : 0);
-		for (int y = 0; y < h; y++) for (int x = 0; x < w; x++) {
-			size_t o = base + (size_t)y * stride + x;
-			if (c->host_out[o] == port[o]) continue;
-			int a = (y / (pl ? 8 : 16)) * W + x / (pl ? 8 : 16);
-			fprintf(stderr, "MISMATCH picture %d (slot %d, %dx%d macroblocks, %d intra) plane %d x %d y %d: device %d port %d\n", pic, dst, W, H, pd.n_intra, pl, x, y, c->host_out[o], port[o]);
-			dump_mb(c, a);
-			return 1;
-		}
+	uint32_t reads = 0;
+	for (int a = 0; a < c->nmb; a++) if (c->recs[a].kind == MBK_INTER)
+		for (int l = 0; l < 2; l++) for (int i8 = 0; i8 < 4; i8++) if (c->recs[a].ref_idx[l][i8] >= 0) reads |= 1u << c->recs[a].ref_pic[l][i8];
+	if (c->inflight > 1) {   /* what this picture shares with the pictures in flight when it is submitted, and whether the staging ring is full */
+		int ref_in = 0, dst_in = 0;
+		for (int k = 0; k < c->n_out; k++) { const Pending *o = c->q + (c->q_head + k) % c->inflight; ref_in |= reads >> o->dst & 1; dst_in |= o->reads >> dst & 1; }
+		cov[C_REF_IN_FLIGHT] += ref_in; cov[C_DST_READ_IN_FLIGHT] += dst_in; cov[C_STAGING_WRAPPED] += c->n_out >= c->n_stage;
 	}
-	return 0;
+	pthread_mutex_lock(&port_mu);
+	port_recon_picture(c->port_frames, &pd, c->recs, c->coefs, c->slices);
+	pthread_mutex_unlock(&port_mu);
+	Pending *p = c->q + (c->q_head + c->n_out) % c->inflight;
+	p->pic = pic; p->dst = dst; p->reads = reads; p->pd = pd;
+	if (++c->n_out > cov[C_INFLIGHT_MAX]) cov[C_INFLIGHT_MAX] = c->n_out;
+	if (c->inflight > 1) c->prev_dst = dst;
+	if (!cpu_only) {
+		memcpy(p->port, c->port_frames + (size_t)dst * c->g.frame_bytes, (size_t)c->g.frame_bytes);
+		memcpy(p->recs, c->recs, (size_t)c->nmb * sizeof(E264MbRec));
+		memcpy(p->coefs, c->coefs, (size_t)pd.n_coefs * 2);
+		memcpy(p->slices, c->slices, (size_t)pd.n_slices * sizeof(E264SliceRec));
+		memcpy(p->intra_list, c->intra_list, (size_t)pd.n_intra * 4);
+	}
+	return c->n_out == c->inflight ? flush(c, cpu_only) : 0;
 }
 
-int main(int argc, char **argv) {
-	int cpu_only = 0, s0 = 1, s1 = 1, pictures = 0, gw = 0, gh = 0;
-	const char *lib = NULL;
-	for (int i = 1; i < argc; i++) {
-		if (!strcmp(argv[i], "--cpu-only")) cpu_only = 1;
-		else if (!strcmp(argv[i], "--lib") && i + 1 < argc) lib = argv[++i];
-		else if (!strcmp(argv[i], "--seeds") && i + 1 < argc) { if (sscanf(argv[++i], "%d-%d", &s0, &s1) == 1) s1 = s0; }
-		else if (!strcmp(argv[i], "--pictures") && i + 1 < argc) pictures = atoi(argv[++i]);
-		else if (!strcmp(argv[i], "--geom") && i + 1 < argc) sscanf(argv[++i], "%dx%d", &gw, &gh);
-		else { fprintf(stderr, "usage: %s [--cpu-only] [--lib path] [--seeds A-B] [--pictures N] [--geom WxH]\n", argv[0]); return 2; }
-	}
-	if (!cpu_only) { if (!lib) { fprintf(stderr, "--lib is needed without --cpu-only\n"); return 2; } load_device(lib); }
-	/* widths around INTER_CHUNK (64) and the row-above staging, heights around IR_ROWS / DBK_PAIRS bands, 1-wide pictures,
-	 * 4096-sample strides, 1080p */
-	static const int geoms[][2] = {{1, 1}, {1, 9}, {9, 1}, {63, 2}, {64, 3}, {65, 2}, {129, 2}, {3, 7}, {4, 8}, {2, 9},
-	                               {3, 15}, {2, 16}, {3, 17}, {2, 33}, {120, 68}, {256, 2}, {5, 4}, {7, 6}};
-	const int n_geoms = sizeof(geoms) / sizeof(geoms[0]);
-	int fails = 0, total = 0;
-	for (int seed = s0; seed <= s1; seed++) {
+/* ---- one host thread per context: seeds first + k * step, one after the other, each on a context from e264b_create ---- */
+static const int geoms[][2] = {{1, 1}, {1, 9}, {9, 1}, {63, 2}, {64, 3}, {65, 2}, {129, 2}, {3, 7}, {4, 8}, {2, 9},
+                               {3, 15}, {2, 16}, {3, 17}, {2, 33}, {120, 68}, {256, 2}, {5, 4}, {7, 6}};
+typedef struct {
+	int first, last, step, cpu_only, pictures, gw, gh, inflight;   /* in */
+	int total, fails;                                             /* out */
+} Job;
+static struct {   /* every context's counters, summed as its thread ends */
+	pthread_mutex_t mu; long cov[C_N]; uint64_t qp_seen[3]; uint8_t intra_seen[4][9][16];
+} all = {PTHREAD_MUTEX_INITIALIZER};
+
+static void *run_context(void *arg) {
+	Job *j = (Job *)arg;
+	const int n_geoms = sizeof(geoms) / sizeof(geoms[0]), K = j->inflight, cpu_only = j->cpu_only;
+	for (int seed = j->first; seed <= j->last; seed += j->step) {
 		rng = 0x9E3779B97F4A7C15ull * (uint64_t)(seed + 1) ^ 0xD1B54A32D192ED03ull;
-		int W = gw ? gw : geoms[seed % n_geoms][0], H = gh ? gh : geoms[seed % n_geoms][1];
+		int W = j->gw ? j->gw : geoms[seed % n_geoms][0], H = j->gh ? j->gh : geoms[seed % n_geoms][1];
 		Ctx c; memset(&c, 0, sizeof(c));
 		geometry(&c, W, H, 2 + rnd(MAX_SLOTS - 1));
-		int n_pics = pictures ? pictures : W * H >= 4096 ? 3 : W * H >= 100 ? 12 : 24;
+		c.inflight = K;
+		if (K > 1) {   /* often fewer staging areas than pictures in flight: e264b_acquire_staging then waits for the oldest */
+			c.g.staging = pct(50) ? K : 2 + rnd(K - 1);
+			c.n_stage = c.g.staging < FUZZ_NSTAGE ? c.g.staging : FUZZ_NSTAGE;
+		}
+		int n_pics = j->pictures ? j->pictures : W * H >= 4096 ? 3 : W * H >= 100 ? 12 : 24;
+		if (K > 1 && !j->pictures) n_pics += 2 * K;
+		c.q = calloc(K, sizeof(Pending));
 		if (!cpu_only) {
-			if (D.create(&c.dev)) { fprintf(stderr, "e264b_create failed\n"); return 3; }
-			if (D.configure(c.dev, &c.g, c.n_slots)) { fprintf(stderr, "e264b_configure failed\n"); return 3; }
-			c.host_out = D.host_alloc(c.dev, c.g.frame_bytes);
+			if (D.create(&c.dev)) { fprintf(stderr, "e264b_create failed\n"); exit(3); }
+			if (D.configure(c.dev, &c.g, c.n_slots)) { fprintf(stderr, "e264b_configure failed\n"); exit(3); }
+			for (int k = 0; k < K; k++) {
+				Pending *p = c.q + k;
+				p->host_out = D.host_alloc(c.dev, c.g.frame_bytes); p->port = malloc(c.g.frame_bytes);
+				p->recs = malloc((size_t)c.nmb * sizeof(E264MbRec)); p->coefs = malloc((size_t)c.coef_cap * 2);
+				p->slices = malloc(MAX_SLICES * sizeof(E264SliceRec)); p->intra_list = malloc((size_t)c.nmb * 4);
+				if (!p->host_out || !p->port || !p->recs || !p->coefs || !p->slices || !p->intra_list) { fprintf(stderr, "out of memory\n"); exit(3); }
+			}
 		}
 		for (int s = 0; s < c.n_slots; s++) {   /* every slot starts identical on both sides */
 			int y = rnd(256), cc = rnd(256);
@@ -453,37 +543,84 @@ int main(int argc, char **argv) {
 			memset(f, y, c.g.plane_y); memset(f + c.g.plane_y, cc, c.g.frame_bytes - c.g.plane_y);
 			if (!cpu_only) D.fill(c.dev, s, y, cc);
 		}
-		int bad = 0;
-		for (int s = 0; s < c.n_slots && !bad; s++) bad = run_picture(&c, total++, s, s % 3, cpu_only);   /* textured references */
-		for (int p = 0; p < n_pics && !bad; p++) bad = run_picture(&c, total++, rnd(c.n_slots), -1, cpu_only);
-		if (bad) { fprintf(stderr, "seed %d (%dx%d, %d slots) failed\n", seed, W, H, c.n_slots); fails++; }
-		if (!cpu_only) { D.host_free(c.dev, c.host_out); D.destroy(c.dev); }
-		free(c.port_alloc); free(c.recs); free(c.coefs); free(c.slices); free(c.intra_list);
+		int bad = 0, first_pic = j->total;
+		for (int s = 0; s < c.n_slots && !bad; s++) bad = run_picture(&c, j->total++, s, s % 3, cpu_only);   /* textured references */
+		for (int p = 0; p < n_pics && !bad; p++) bad = run_picture(&c, j->total++, draw_dst(&c), -1, cpu_only);
+		if (c.n_out && !bad) bad = flush(&c, cpu_only);
+		if (!cpu_only && c.n_out) D.wait(c.dev, c.q[(c.q_head + c.n_out - 1) % K].ticket);   /* after a mismatch: nothing left writing into host_out */
+		if (!cpu_only && !bad && D.error_flag(c.dev)) { fprintf(stderr, "device error word %d\n", D.error_flag(c.dev)); bad = 1; }
+		if (bad) { fprintf(stderr, "seed %d (%dx%d, %d slots, pictures %d-%d, %d in flight, %d staging) failed\n", seed, W, H, c.n_slots, first_pic, j->total - 1, K, c.n_stage); j->fails++; }
+		if (!cpu_only) {
+			for (int k = 0; k < K; k++) { Pending *p = c.q + k; D.host_free(c.dev, p->host_out); free(p->port); free(p->recs); free(p->coefs); free(p->slices); free(p->intra_list); }
+			D.destroy(c.dev);
+		}
+		free(c.q); free(c.port_alloc); free(c.recs); free(c.coefs); free(c.slices); free(c.intra_list);
 	}
+	pthread_mutex_lock(&all.mu);
+	for (int i = 0; i < C_N; i++) all.cov[i] = i == C_INFLIGHT_MAX ? (cov[i] > all.cov[i] ? cov[i] : all.cov[i]) : all.cov[i] + cov[i];
+	for (int i = 0; i < 3; i++) all.qp_seen[i] |= qp_seen[i];
+	for (int k = 0; k < 4; k++) for (int m = 0; m < 9; m++) for (int u = 0; u < 16; u++) all.intra_seen[k][m][u] |= intra_seen[k][m][u];
+	pthread_mutex_unlock(&all.mu);
+	return NULL;
+}
+
+int main(int argc, char **argv) {
+	int cpu_only = 0, s0 = 1, s1 = 1, pictures = 0, gw = 0, gh = 0, M = 1, K = 1;
+	const char *lib = NULL;
+	for (int i = 1; i < argc; i++) {
+		if (!strcmp(argv[i], "--cpu-only")) cpu_only = 1;
+		else if (!strcmp(argv[i], "--lib") && i + 1 < argc) lib = argv[++i];
+		else if (!strcmp(argv[i], "--seeds") && i + 1 < argc) { if (sscanf(argv[++i], "%d-%d", &s0, &s1) == 1) s1 = s0; }
+		else if (!strcmp(argv[i], "--pictures") && i + 1 < argc) pictures = atoi(argv[++i]);
+		else if (!strcmp(argv[i], "--geom") && i + 1 < argc) sscanf(argv[++i], "%dx%d", &gw, &gh);
+		else if (!strcmp(argv[i], "--contexts") && i + 1 < argc) M = atoi(argv[++i]);
+		else if (!strcmp(argv[i], "--inflight") && i + 1 < argc) K = atoi(argv[++i]);
+		else { fprintf(stderr, "usage: %s [--cpu-only] [--lib path] [--seeds A-B] [--pictures N] [--geom WxH] [--contexts M] [--inflight K]\n", argv[0]); return 2; }
+	}
+	if (M < 1 || K < 1 || s1 < s0) { fprintf(stderr, "--contexts and --inflight take at least 1, --seeds A-B needs A <= B\n"); return 2; }
+	if (M > s1 - s0 + 1) M = s1 - s0 + 1;
+	if (!cpu_only) { if (!lib) { fprintf(stderr, "--lib is needed without --cpu-only\n"); return 2; } load_device(lib); }
+	/* widths around INTER_CHUNK (64) and the row-above staging, heights around IR_ROWS / DBK_PAIRS bands, 1-wide pictures,
+	 * 4096-sample strides, 1080p: the list geoms above, seed k takes geometry k % 18 */
+	Job *jobs = calloc(M, sizeof(Job));
+	pthread_t *th = calloc(M, sizeof(pthread_t));
+	for (int t = 0; t < M; t++) {
+		jobs[t] = (Job){s0 + t, s1, M, cpu_only, pictures, gw, gh, K, 0, 0};
+		if (pthread_create(th + t, NULL, run_context, jobs + t)) { fprintf(stderr, "pthread_create failed\n"); return 3; }
+	}
+	int fails = 0, total = 0;
+	for (int t = 0; t < M; t++) { pthread_join(th[t], NULL); fails += jobs[t].fails; total += jobs[t].total; }
+	const int concurrent = M > 1 || K > 1;
+	if (concurrent) for (int t = 0; t < M; t++) printf("context %d: %d pictures, %d failing seeds\n", t, jobs[t].total, jobs[t].fails);
+	all.cov[C_CONTEXTS] = M;
 	int combos = 0;
-	for (int k = 0; k < 4; k++) for (int m = 0; m < 9; m++) for (int u = 0; u < 16; u++) combos += intra_seen[k][m][u] != 0;
-	cov[C_INTRA_COMBOS] = combos;
-	cov[C_QPY] = __builtin_popcountll(qp_seen[0]); cov[C_QPCB] = __builtin_popcountll(qp_seen[1]); cov[C_QPCR] = __builtin_popcountll(qp_seen[2]);
+	for (int k = 0; k < 4; k++) for (int m = 0; m < 9; m++) for (int u = 0; u < 16; u++) combos += all.intra_seen[k][m][u] != 0;
+	all.cov[C_INTRA_COMBOS] = combos;
+	all.cov[C_QPY] = __builtin_popcountll(all.qp_seen[0]); all.cov[C_QPCB] = __builtin_popcountll(all.qp_seen[1]); all.cov[C_QPCR] = __builtin_popcountll(all.qp_seen[2]);
 	static const char *names[C_N] = {"qp_y_values", "qp_cb_values", "qp_cr_values", "level_32767", "level_-32768", "scaling_flat16", "scaling_all255",
 		"scaling_all1", "scaling_random", "weight_-128", "weight_127", "weight_128_uni_logwd7", "offset_-128", "offset_127", "explicit_logwd0",
 		"explicit_logwd7", "implicit_w1_-64", "implicit_w1_128", "implicit_w1_other", "one_picture_two_weights", "mv_int16_extreme", "mv_near_border",
 		"dmv_x_3", "dmv_x_4", "dmv_y_3", "dmv_y_4", "same_picture_both_lists", "swapped_lists", "one_list_vs_two"};
-	for (int i = 0; i < C_N; i++) {
+	for (int i = 0; i <= C_PICTURES; i++) {
 		if (i >= C_BS && i < C_BS + 30) {
 			int e = (i - C_BS) / 10, bs = (i - C_BS) % 5;
 			if ((e < 2 && bs == 3) || (e == 2 && bs == 4)) continue;   /* macroblock edges take 4 where internal edges take 3 */
-			printf("cov %s %ld\n", bs_name(i - C_BS), cov[i]);
+			printf("cov %s %ld\n", bs_name(i - C_BS), all.cov[i]);
 			continue;
 		}
 		if (i >= C_BS + 30 && i < C_FOFF_M12) continue;
 		static const char *tail[] = {"filter_offset_-12", "filter_offset_12", "deblock_idc_0", "deblock_idc_1", "deblock_idc_2", "slices_64",
 			"intra_mode_availability_pairs", "ipcm", "conceal_inter", "conceal_intra", "intra_fraction_0", "intra_fraction_1",
 			"intra_fraction_below_half", "intra_fraction_half", "intra_fraction_above_half", "intra_fraction_all", "explicit_bi_logwd7_bright", "pictures"};
-		printf("cov %s %ld\n", i < C_BS ? names[i] : tail[i - C_FOFF_M12], cov[i]);
+		printf("cov %s %ld\n", i < C_BS ? names[i] : tail[i - C_FOFF_M12], all.cov[i]);
 	}
 	static const char *res[6] = {"sat16_4x4", "wrap_8x8_div_lt6", "wrap_8x8_div_ge6", "wrap_luma_dc32", "chroma_dc_qpc39", "wrap16_dc_only"};
 	for (int i = 0; i < 6; i++) printf("cov %s %ld\n", res[i], port_cov_residual[i]);
 	printf("cov wp_bi_sat16 %ld\n", port_cov_wp_bi_sat16);
+	if (concurrent) {
+		static const char *inflight_names[] = {"inflight_max", "ref_slot_in_flight", "dst_slot_read_in_flight", "staging_wrapped", "contexts"};
+		for (int i = C_INFLIGHT_MAX; i < C_N; i++) printf("cov %s %ld\n", inflight_names[i - C_INFLIGHT_MAX], all.cov[i]);
+	}
 	printf("%d pictures, %d failing seeds\n", total, fails);
 	return fails ? 1 : 0;
 }

@@ -21,7 +21,7 @@ SEEDS = "0-35"
 @pytest.fixture(scope="module")
 def fuzzer(tmp_path_factory):
     exe = str(tmp_path_factory.mktemp("fuzz") / "record_fuzz")
-    subprocess.run(["gcc", "-O2", "-std=gnu11", "-w"] + FUZZ_SRC + ["-o", exe, "-ldl"], check=True)
+    subprocess.run(["gcc", "-O2", "-std=gnu11", "-w", "-pthread"] + FUZZ_SRC + ["-o", exe, "-ldl"], check=True)
     return exe
 
 
