@@ -73,6 +73,8 @@ def bind(path):
     if hasattr(lib, "edge264_get_packed"):     # the extension of include/edge264_packed.h
         lib.edge264_enable_packed.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
         lib.edge264_get_packed.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264Packed)]
+    if hasattr(lib, "edge264_enable_resized"):   # the resized output of include/edge264_packed.h
+        lib.edge264_enable_resized.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     if hasattr(lib, "edge264_set_skip"):       # the extension of include/edge264_skip.h
         lib.edge264_set_skip.argtypes = [ctypes.c_void_p, ctypes.c_int]
     _loaded[path] = lib
@@ -153,12 +155,13 @@ def frame_packed(lib, dec, f):
     return out
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE):
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
     carries the frame's motion export (frame_motion); with packed=(format, log2_scale) it ends with the frame's packed
-    output (frame_packed); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip)."""
+    output (frame_packed); resized=(format, width, height) does the same with the resized output (edge264_enable_resized,
+    log2_scale -1); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip)."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -179,6 +182,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             d = ctypes.c_void_p(dec)
             lib.edge264_free(ctypes.byref(d))
             raise RuntimeError("edge264_enable_packed: %s" % errno.errorcode.get(r, r))
+    if resized is not None:
+        r = lib.edge264_enable_resized(dec, *resized) if hasattr(lib, "edge264_enable_resized") else errno.ENOTSUP
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_enable_resized: %s" % errno.errorcode.get(r, r))
     if skip != SKIP_NONE:
         r = lib.edge264_set_skip(dec, skip) if hasattr(lib, "edge264_set_skip") else errno.ENOTSUP
         if r:
@@ -196,7 +205,7 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             drained = True
         while lib.edge264_get_frame(dec, ctypes.byref(f), 0) == 0:
             frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ())
-                          + ((frame_motion(lib, dec, f),) if motion else ()) + ((frame_packed(lib, dec, f),) if packed is not None else ()))
+                          + ((frame_motion(lib, dec, f),) if motion else ()) + ((frame_packed(lib, dec, f),) if packed is not None or resized is not None else ()))
         if res == errno.ENOBUFS:
             if len(frames) == before:
                 break

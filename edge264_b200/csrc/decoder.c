@@ -251,11 +251,21 @@ static void hostbuf_free(Edge264Decoder *d, HostBuf *hb) {
 	}
 	memset(hb, 0, sizeof(*hb));
 }
-/* what the pictures of the active sequence are packed as: the decoder's format and scale, the sequence's cropping rectangle */
+/* the nearest even size to s_a * t_b / s_b, within 2..16384: the resized side that keeps the aspect ratio */
+static int32_t aspect_size(int64_t s_a, int64_t s_b, int64_t t_b) {
+	const int64_t t = 2 * ((s_a * t_b + s_b) / (2 * s_b));
+	return (int32_t)(t < 2 ? 2 : t > 16384 ? 16384 : t);
+}
+/* what the pictures of the active sequence are packed as: the decoder's format and scale, the sequence's cropping
+ * rectangle, and for the resized output the requested size, a 0 side derived from the cropping rectangle */
 static E264PackedDesc packed_desc(const Edge264Decoder *d) {
 	const Edge264Frame *o = &d->out_fmt;
 	E264PackedDesc k = {d->packed_format, d->packed_scale, o->frame_crop_offsets[3], o->frame_crop_offsets[0],
 	                    d->w_mbs * 16 - o->frame_crop_offsets[3] - o->frame_crop_offsets[1], d->h_mbs * 16 - o->frame_crop_offsets[0] - o->frame_crop_offsets[2]};
+	if (d->packed_scale < 0) {
+		k.target_width = d->packed_width ? d->packed_width : aspect_size(k.width, k.height, d->packed_height);
+		k.target_height = d->packed_height ? d->packed_height : aspect_size(k.height, k.width, d->packed_width);
+	}
 	return k;
 }
 /* a buffer beside the samples, of their memory kind: from the application's allocator, else from the backend's output
@@ -1366,6 +1376,15 @@ int edge264_enable_packed(Edge264Decoder *d, int format, int log2_scale) {
 	if (!d->be->submit_outputs) return ENOTSUP;
 	if (d->slices_seen) return EBUSY;   /* host buffers are created with the first picture: they would lack the packed one */
 	d->packed = 1; d->packed_format = format; d->packed_scale = log2_scale;
+	return 0;
+}
+
+int edge264_enable_resized(Edge264Decoder *d, int format, int width, int height) {
+	if (!d || (format != EDGE264_PACKED_I420 && format != EDGE264_PACKED_NV12) || ((width | height) & 1) || width < 0 || height < 0 ||
+	    width > 16384 || height > 16384 || (width | height) == 0) return EINVAL;
+	if (!d->be->submit_outputs) return ENOTSUP;
+	if (d->slices_seen) return EBUSY;   /* host buffers are created with the first picture: they would lack the resized one */
+	d->packed = 1; d->packed_format = format; d->packed_scale = -1; d->packed_width = width; d->packed_height = height;
 	return 0;
 }
 

@@ -22,6 +22,7 @@
 #include "intra_kernels.cuh"
 #include "motion_kernels.cuh"
 #include "pack_kernels.cuh"
+#include "resize_kernels.cuh"
 extern "C" {
 #include "dec.h"
 }
@@ -359,6 +360,33 @@ static int pack_picture(E264bDevice *c, const E264PicDesc *pd, const E264PackedD
 	return 0;
 }
 
+/* the resized output of the picture in frame slot pd->dst_slot into d_packed: one launch over all planes */
+static int resize_picture(E264bDevice *c, const E264PicDesc *pd, const E264PackedDesc *pk, const E264PackedLayout &L) {
+	const uint8_t *slot = c->d_frames + (size_t)pd->dst_slot * pd->frame_bytes;
+	const bool nv12 = pk->format == E264_PACKED_NV12;
+	ResizeArgs A; memset(&A, 0, sizeof(A));
+	int blocks = 0;
+	for (int i = 0; i < (nv12 ? 2 : 3); i++) {
+		ResizePlane &P = A.p[i];
+		if (i == 0) { P.src = slot + (size_t)pk->top * pd->stride_y + pk->left; P.src_stride = pd->stride_y; P.sw = pk->width; P.sh = pk->height; P.tw = L.width; P.th = L.height; }
+		else {
+			P.src = slot + pd->plane_y + (size_t)(pk->top >> 1) * pd->stride_c + (pk->left >> 1) + (i == 2 ? pd->stride_c >> 1 : 0);
+			P.src_stride = pd->stride_c; P.sw = pk->width >> 1; P.sh = pk->height >> 1; P.tw = L.width_C; P.th = L.height_C;
+		}
+		P.dst = c->d_packed + L.offset[i]; P.dst_stride = L.stride[i];
+		P.inv = e264_rs_inv((int64_t)P.sw * P.sh);
+		P.bx = (P.tw + RS_TW - 1) / RS_TW; P.first = blocks;
+		blocks += P.bx * ((P.th + RS_TH - 1) / RS_TH);
+	}
+	if (nv12) A.p[2].first = blocks;
+	A.cr_off = pd->stride_c >> 1;
+	if (nv12) e264_resize_kernel<E264_PACKED_NV12><<<blocks, RS_THREADS, 0, c->stream>>>(A);
+	else e264_resize_kernel<E264_PACKED_I420><<<blocks, RS_THREADS, 0, c->stream>>>(A);
+	c->launches++;
+	CK(cudaGetLastError());
+	return 0;
+}
+
 static int is_device_memory(const void *p) {
 	cudaPointerAttributes a;
 	const int dev = cudaPointerGetAttributes(&a, p) == cudaSuccess && a.type == cudaMemoryTypeDevice;
@@ -381,8 +409,12 @@ extern "C" int e264b_submit_outputs(E264bDevice *c, const E264PicDesc *pd, uint8
 	E264PackedLayout pl; memset(&pl, 0, sizeof(pl));
 	if (packed) {
 		const E264PackedDesc *k = &o->pk;
-		if ((k->format != E264_PACKED_I420 && k->format != E264_PACKED_NV12) || k->log2_scale < 0 || k->log2_scale > 3 || ((k->left | k->top | k->width | k->height) & 1) ||
+		const bool resized = k->target_width || k->target_height;
+		if ((k->format != E264_PACKED_I420 && k->format != E264_PACKED_NV12) || ((k->left | k->top | k->width | k->height) & 1) ||
 		    k->left < 0 || k->top < 0 || k->width < 2 || k->height < 2 || k->left + k->width > pd->width_mbs * 16 || k->top + k->height > pd->height_mbs * 16) return -1;
+		if (resized ? k->log2_scale != -1 || ((k->target_width | k->target_height) & 1) || k->target_width < 2 || k->target_height < 2 ||
+		              k->target_width > 16384 || k->target_height > 16384 || (int64_t)k->width * k->height >= (1 << 29)   /* resize_math.cuh */
+		            : k->log2_scale < 0 || k->log2_scale > 3) return -1;
 		pl = e264_packed_layout(k);
 	}
 	CK(cudaSetDevice(c->dev));
@@ -431,7 +463,7 @@ extern "C" int e264b_submit_outputs(E264bDevice *c, const E264PicDesc *pd, uint8
 			c->d_packed = NULL; c->packed_cap = 0;
 			CK(cudaMalloc(&c->d_packed, pl.bytes)); c->packed_cap = pl.bytes;
 		}
-		if (pack_picture(c, pd, &o->pk, pl)) return -1;
+		if ((o->pk.target_width ? resize_picture(c, pd, &o->pk, pl) : pack_picture(c, pd, &o->pk, pl))) return -1;
 		CK(cudaMemcpyAsync(packed, c->d_packed, pl.bytes, cudaMemcpyDefault, c->stream)); c->d2h_bytes += pl.bytes;
 		if (o->packed_on_device) *o->packed_on_device = is_device_memory(packed);
 	}

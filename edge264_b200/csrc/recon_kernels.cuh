@@ -7,6 +7,7 @@
  *   deblock_kernels.cuh  e264_deblock_kernel     boundary strengths + the in-loop filter: band wavefront
  *   motion_kernels.cuh   e264_motion_kernel      the motion export (decoders that asked for it): records -> raster arrays
  *   pack_kernels.cuh     e264_pack_kernel        the packed output (decoders that asked for it): frame slot -> cropped I420 / NV12, box-downscaled
+ *   resize_kernels.cuh   e264_resize_kernel      the resized output (decoders that asked for it): frame slot -> cropped I420 / NV12, any size, area-averaged
  * Up to three launches per picture.  Arithmetic is restated from ITU-T H.264 with the reference's observable integer
  * widths; results are bit-exact with the reference decoder (tests/test_gpu_parity.py). */
 #pragma once

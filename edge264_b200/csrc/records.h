@@ -138,12 +138,14 @@ typedef struct E264PicDesc {
 enum { E264_MOTION_MV = 0, E264_MOTION_REF = 128, E264_MOTION_TYPE = 160, E264_MOTION_QP = 161, E264_MOTION_BYTES = 162 };
 
 /* The packed output of one picture (include/edge264_packed.h): the cropped picture as I420 or NV12, box-downscaled by
- * 1 << log2_scale, in one buffer.  E264PackedDesc says what to pack, e264_packed_layout where every plane goes: sizes are
- * ceil(cropped size / scale), a row stride is the row's bytes rounded up to 64, a plane starts on a multiple of 256. */
+ * 1 << log2_scale, or resized to target_width x target_height, in one buffer.  E264PackedDesc says what to pack,
+ * e264_packed_layout where every plane goes: sizes are ceil(cropped size / scale), or the target (chroma: half of it), a
+ * row stride is the row's bytes rounded up to 64, a plane starts on a multiple of 256. */
 enum { E264_PACKED_I420 = 0, E264_PACKED_NV12 = 1 };
 typedef struct E264PackedDesc {
-	int32_t format, log2_scale;         /* E264_PACKED_*, 0..3 */
+	int32_t format, log2_scale;         /* E264_PACKED_*, 0..3, or -1 for the resized output */
 	int32_t left, top, width, height;   /* the cropping rectangle inside the coded picture, luma samples (all even: 4:2:0 frames) */
+	int32_t target_width, target_height;   /* resized output: the luma size, even, 2..16384; 0, 0 in the power-of-two mode */
 } E264PackedDesc;
 typedef struct E264PackedLayout {
 	int32_t width, height, width_C, height_C;   /* samples per plane after cropping and scaling */
@@ -151,10 +153,14 @@ typedef struct E264PackedLayout {
 	int32_t bytes;                              /* size of the buffer */
 } E264PackedLayout;
 static inline E264PackedLayout e264_packed_layout(const E264PackedDesc *p) {
-	const int n = 1 << p->log2_scale;
 	E264PackedLayout l;
-	l.width = (p->width + n - 1) >> p->log2_scale; l.height = (p->height + n - 1) >> p->log2_scale;
-	l.width_C = ((p->width >> 1) + n - 1) >> p->log2_scale; l.height_C = ((p->height >> 1) + n - 1) >> p->log2_scale;
+	if (p->target_width) {
+		l.width = p->target_width; l.height = p->target_height; l.width_C = l.width >> 1; l.height_C = l.height >> 1;
+	} else {
+		const int n = 1 << p->log2_scale;
+		l.width = (p->width + n - 1) >> p->log2_scale; l.height = (p->height + n - 1) >> p->log2_scale;
+		l.width_C = ((p->width >> 1) + n - 1) >> p->log2_scale; l.height_C = ((p->height >> 1) + n - 1) >> p->log2_scale;
+	}
 	l.stride[0] = (l.width + 63) & ~63;
 	l.stride[1] = ((p->format == E264_PACKED_NV12 ? 2 * l.width_C : l.width_C) + 63) & ~63;
 	l.stride[2] = p->format == E264_PACKED_NV12 ? 0 : l.stride[1];

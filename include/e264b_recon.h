@@ -45,8 +45,9 @@ int   e264b_submit_motion(E264bDevice *dev, const struct E264PicDesc *pic, uint8
                           const int32_t *slot_ids, int n_ids, int *on_device, uint64_t *ticket);
 /* The one submit the three above are thin callers of: `out` (struct E264Outputs of edge264_b200/csrc/records.h) names the
  * optional outputs, each left out when its pointer is NULL: the error map, the motion export, and the packed output
- * (include/edge264_packed.h: the cropped picture as I420 or NV12, optionally box-downscaled, written by e264_pack_kernel
- * with the layout of e264_packed_layout; one launch and one copy of that many bytes per picture). */
+ * (include/edge264_packed.h: the cropped picture as I420 or NV12, optionally box-downscaled, written by e264_pack_kernel,
+ * or resized to out->pk's target size by exact area averaging, written by e264_resize_kernel; with the layout of
+ * e264_packed_layout; one launch and one copy of that many bytes per picture). */
 int   e264b_submit_outputs(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, const struct E264Outputs *out, uint64_t *ticket);
 int   e264b_wait(E264bDevice *dev, uint64_t ticket);
 int   e264b_poll(E264bDevice *dev, uint64_t ticket);          /* 0 complete, EAGAIN still on the device, < 0 device error */
