@@ -57,22 +57,6 @@ __device__ __forceinline__ void mc_load_chroma(const uint8_t *plane, int stride,
 	}
 }
 
-/* 8.4.2.3 on four packed samples in ONE form: (sat16(a * wa + b * wb + rnd) >> sh) + o, clipped.  Implicit bi-prediction:
- * wa = w0, wb = w1, rnd = 2^logWD, sh = logWD + 1, o = 0; explicit bi-prediction: the same with the offsets folded into
- * rnd = ((o0 + o1 + 1) | 1) << logWD and o = 0, saturated to int16 as the reference does (edge264_inter.c:17-29,
- * :1176-1178; it differs from the standard only at logWD 7, oracle/port_recon.c wp_bi); explicit weighting of a single
- * prediction: wa = w, wb = 0, rnd = 2^(logWD-1) (0 when logWD = 0), sh = logWD.  Only explicit bi-prediction can reach the
- * saturation (reference edge264_inter.c:1140-1180 keeps five variants). */
-__device__ __forceinline__ uint32_t wp_word(uint32_t a, uint32_t b, int wa, int wb, int rnd, int sh, int o) {
-	uint32_t r = 0;
-#pragma unroll
-	for (int k = 0; k < 4; k++) {
-		const int pa = (a >> (8 * k)) & 255, pb = (b >> (8 * k)) & 255;
-		r |= (uint32_t)mc_clip255((min(max(pa * wa + pb * wb + rnd, -32768), 32767) >> sh) + o) << (8 * k);
-	}
-	return r;
-}
-
 /* ---- the kernel ----
  * A block takes chunks of INTER_CHUNK consecutive macroblocks.  Per chunk:
  *   1. records into shared memory; every (macroblock, list, 4x4 block) that is predicted becomes an ITEM and is queued by

@@ -6,8 +6,10 @@
  * (dp4a: taps 1,-5,20,20 | -5,1,0,0 against byte windows cut out with funnel shifts); the vertical cases run the same
  * code on the transposed window (byte-permute 4x4 transposes) — the interpolation is symmetric under transposition,
  * including the reference's order of passes for the centre sample (vertical first when xFrac is odd, edge264_inter.c:
- * 559-640), whose wrapping int16 combination (edge264_inter.c:4-9) is reproduced bit for bit.
- * Host-compilable: tests/mc_math_check.cpp runs these functions against the oracle's per-sample restatement. */
+ * 559-640), whose wrapping int16 combination (edge264_inter.c:4-9) is reproduced bit for bit.  The weighted combination
+ * of the predictions (8.4.2.3) is here too.
+ * Host-compilable: tests/mc_math_check.cpp runs these functions against the oracle's per-sample restatement, and
+ * tests/test_pixel_spec.py runs the chroma interpolation and the weighting against the standard's equations in numpy. */
 #pragma once
 #include <stdint.h>
 
@@ -38,6 +40,23 @@ MC_FN uint32_t mc_add_res4(uint32_t p, uint32_t r01, uint32_t r23) {
 }
 /* rounded-up average of four bytes at once */
 MC_FN uint32_t mc_avg4(uint32_t a, uint32_t b) { return (a | b) - (((a ^ b) >> 1) & 0x7f7f7f7fu); }
+
+/* 8.4.2.3 on four packed samples in ONE form: (sat16(a * wa + b * wb + rnd) >> sh) + o, clipped.  Implicit bi-prediction:
+ * wa = w0, wb = w1, rnd = 2^logWD, sh = logWD + 1, o = 0; explicit bi-prediction: the same with the offsets folded into
+ * rnd = ((o0 + o1 + 1) | 1) << logWD and o = 0, saturated to int16 as the reference does (edge264_inter.c:17-29,
+ * :1176-1178; it differs from the standard only at logWD 7, oracle/port_recon.c wp_bi, counted by
+ * tests/test_pixel_spec.py); explicit weighting of a single prediction: wa = w, wb = 0, rnd = 2^(logWD-1) (0 when
+ * logWD = 0), sh = logWD.  Only explicit bi-prediction can reach the saturation (reference edge264_inter.c:1140-1180 keeps
+ * five variants). */
+MC_FN uint32_t wp_word(uint32_t a, uint32_t b, int wa, int wb, int rnd, int sh, int o) {
+	uint32_t r = 0;
+#pragma unroll
+	for (int k = 0; k < 4; k++) {
+		const int pa = (a >> (8 * k)) & 255, pb = (b >> (8 * k)) & 255, s = pa * wa + pb * wb + rnd, lo = s < -32768 ? -32768 : s;
+		r |= (uint32_t)mc_clip255(((lo > 32767 ? 32767 : lo) >> sh) + o) << (8 * k);
+	}
+	return r;
+}
 
 /* six-tap sums (1,-5,20,20,-5,1) at the four sample positions x = 0..3 of a row whose samples x = -2..9 are the
  * bytes of (w0, w1, w2): s[x] = p[x-2] - 5 p[x-1] + 20 p[x] + 20 p[x+1] - 5 p[x+2] + p[x+3] */

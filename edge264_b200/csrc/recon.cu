@@ -814,6 +814,51 @@ extern "C" int e264b_kat(int fn, int mode, const uint8_t *in, int in_bytes, uint
 	return 0;
 }
 
+/* ---- batched intra entry point (tests/test_pixel_spec.py -m gpu): many neighbourhoods through the device's intra
+ * predictors in ONE launch, a block per draw.  Draw i has two borders of 33 bytes at borders + 66 i, each p[-1,-1],
+ * p[0..15,-1], p[-1,0..15]; luma (fn 0-2) reads the first, chroma (fn 3) predicts Cb from the first and Cr from the second
+ * (8 samples of each side).  modes[i] = prediction mode | unavailable bits << 4 of Intra4x4 / Intra8x8 block 0 (the other
+ * blocks take DC), of the Intra16x16 macroblock or of both chroma blocks.  out + 256 i receives the 16x16 luma macroblock,
+ * or the 8x8 Cb then Cr blocks. */
+__global__ void e264_kat_batch_kernel(int fn, const uint8_t *modes, const uint8_t *borders, uint8_t *out) {
+	__shared__ WarpSmem wsm;
+	__shared__ E264MbRec rec;
+	WarpSmem *ws = &wsm;
+	const int lane = threadIdx.x, imode = modes[blockIdx.x];
+	const uint8_t *b = borders + (size_t)blockIdx.x * 66;
+	uint8_t *o = out + (size_t)blockIdx.x * 256;
+	for (int i = lane; i < 384; i += 32) ws->res[i] = 0;
+	if (lane == 0) { memset(&rec, 0, sizeof(rec)); rec.kind = fn == 0 ? MBK_I4x4 : fn == 1 ? MBK_I8x8 : MBK_I16x16; for (int k = 0; k < 16; k++) rec.modes[k] = IMODE(2, 0); rec.modes[0] = (uint8_t)imode; rec.i16_mode = (uint8_t)imode; rec.chroma_mode = (uint8_t)imode; }
+	__syncwarp();
+	if (fn < 3) {
+		for (int x = lane - 1; x < 24; x += 32) YT(x, -1) = b[1 + min(x, 15)];
+		if (lane < 16) YT(-1, lane) = b[17 + lane];
+		__syncwarp();
+		intra_luma(ws, &rec, lane);
+		__syncwarp();
+		for (int i = lane; i < 256; i += 32) o[i] = YT(i & 15, i >> 4);
+	} else {
+		if (lane < 18) { const int pl = lane / 9, x = lane % 9 - 1; CT(pl, x, -1) = b[pl * 33 + 1 + x]; }
+		if (lane < 16) { const int pl = lane >> 3, y = lane & 7; CT(pl, -1, y) = b[pl * 33 + 17 + y]; }
+		__syncwarp();
+		intra_chroma(ws, &rec, lane);
+		__syncwarp();
+		for (int i = lane; i < 128; i += 32) o[i] = CT(i >> 6, i & 7, (i >> 3) & 7);
+	}
+}
+extern "C" int e264b_kat_batch(int fn, const uint8_t *modes, const uint8_t *borders, int n, uint8_t *out) {
+	if (fn < 0 || fn > 3 || n <= 0) return -1;
+	uint8_t *d = NULL;
+	CK(cudaMalloc(&d, (size_t)n * (1 + 66 + 256)));
+	uint8_t *d_modes = d, *d_borders = d + n, *d_out = d + (size_t)n * 67;
+	CK(cudaMemcpy(d_modes, modes, n, cudaMemcpyHostToDevice)); CK(cudaMemcpy(d_borders, borders, (size_t)n * 66, cudaMemcpyHostToDevice));
+	e264_kat_batch_kernel<<<n, 32>>>(fn, d_modes, d_borders, d_out);
+	CK(cudaGetLastError()); CK(cudaDeviceSynchronize());
+	CK(cudaMemcpy(out, d_out, (size_t)n * 256, cudaMemcpyDeviceToHost));
+	cudaFree(d);
+	return 0;
+}
+
 /* ---- backend vtable for decoder.c ---- */
 static int be_create(void **ctx) { return e264b_create((E264bDevice **)ctx); }
 static void be_destroy(void *ctx) { e264b_destroy((E264bDevice *)ctx); }

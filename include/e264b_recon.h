@@ -76,6 +76,8 @@ long long e264b_picture_bytes(E264bDevice *dev);              /* width x height 
 int      e264b_replay_frames(E264bDevice *dev, uint8_t *out);  /* every kept picture once more, in decode order, into out */
 /* known-answer support (tests): one block through the device's intra predictors (fn 0-3) or luma interpolation (fn 4) */
 int      e264b_kat(int fn, int mode, const uint8_t *in, int in_bytes, uint8_t *out, int w, int h);
+/* the intra predictors (fn 0-3) over n draws in one launch: modes[n], borders 66 bytes and out 256 bytes per draw (recon.cu) */
+int      e264b_kat_batch(int fn, const uint8_t *modes, const uint8_t *borders, int n, uint8_t *out);
 E264bDevice *e264b_of_decoder(struct Edge264Decoder *dec);
 
 #ifdef __cplusplus
