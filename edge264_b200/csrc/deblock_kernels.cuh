@@ -1,5 +1,7 @@
 /* deblock_kernels.cuh — the in-loop filter (8.7).
  *
+ * The arithmetic of one edge segment (dbk_bs_pair) and of one line of samples (dbk_line_luma, dbk_line_chroma) is in
+ * dbk_math.cuh, which also compiles for the host.
  *   dbk_digest_mb         a 64-byte E264DbkMb per macroblock: 32 boundary strengths (one lane per edge segment), alpha /
  *                         beta / tC0 of the 9 plane x edge-kind combinations (reference: deblock_mb's bS derivation
  *                         and table look-ups, edge264_deblock.c:530-1123) — record-only work without dependencies, a
@@ -22,6 +24,7 @@
  */
 #pragma once
 #include "recon_kernels.cuh"
+#include "dbk_math.cuh"
 
 struct __align__(16) E264DbkMb {
 	uint32_t bs[4];          /* [0..1] vertical edges, [2..3] horizontal edges: nibble (edge * 4 + segment) = bS 0..4 */
@@ -30,32 +33,6 @@ struct __align__(16) E264DbkMb {
 	uint8_t tc0[27];         /* [(plane * 3 + kind) * 3 + bS - 1] */
 	uint8_t pad[3];
 };                           /* 64 bytes */
-
-__device__ __forceinline__ int dbk_iabs(int v) { return v < 0 ? -v : v; }
-
-/* 8.7.2.1 for one edge segment between 4x4 blocks bp of p and bq of q.  Every candidate outcome is computed and the result
- * is selected, so the 32 lanes of a digest (different edges, different cases) run one instruction stream; the records
- * are read whole even where they do not matter (intra macroblocks), which is harmless. */
-__device__ __forceinline__ bool dbk_far(uint32_t a, uint32_t b) {      /* two packed quarter-sample vectors differ by 4 or more */
-	return dbk_iabs((int)(short)(a & 0xffffu) - (int)(short)(b & 0xffffu)) >= 4 || dbk_iabs((int)(short)(a >> 16) - (int)(short)(b >> 16)) >= 4;
-}
-__device__ __forceinline__ int dbk_bs_pair(const E264MbRec *p, int bp, const E264MbRec *q, int bq, bool mb_edge) {
-	const bool intra = p->kind != MBK_INTER || q->kind != MBK_INTER;
-	const bool coef = (((p->coded >> bp) | (q->coded >> bq)) & 1) != 0;
-	const int ip = bp >> 2, iq = bq >> 2;
-	const int p0 = p->ref_idx[0][ip] < 0 ? -1 : p->ref_pic[0][ip], p1 = p->ref_idx[1][ip] < 0 ? -1 : p->ref_pic[1][ip];
-	const int q0 = q->ref_idx[0][iq] < 0 ? -1 : q->ref_pic[0][iq], q1 = q->ref_idx[1][iq] < 0 ? -1 : q->ref_pic[1][iq];
-	const bool same = (p0 == q0 && p1 == q1) || (p0 == q1 && p1 == q0);
-	const uint32_t pm0 = *(const uint32_t *)p->mv[0][bp], pm1 = *(const uint32_t *)p->mv[1][bp];
-	const uint32_t qm0 = *(const uint32_t *)q->mv[0][bq], qm1 = *(const uint32_t *)q->mv[1][bq];
-	const bool f00 = dbk_far(pm0, qm0), f11 = dbk_far(pm1, qm1), f01 = dbk_far(pm0, qm1), f10 = dbk_far(pm1, qm0);
-	const bool straight = f00 || f11, crossed = f01 || f10;
-	/* both lists: distinct pictures pair the vectors by picture, the same picture twice needs both pairings to differ;
-	 * one list: the vectors of the lists in use */
-	const bool one = p0 >= 0 ? (q0 >= 0 ? f00 : f01) : (q0 >= 0 ? f10 : f11);
-	const bool mv = p0 >= 0 && p1 >= 0 ? (p0 != p1 ? (p0 == q0 ? straight : crossed) : straight && crossed) : one;
-	return intra ? (mb_edge ? 4 : 3) : coef ? 2 : !same ? 1 : (int)mv;
-}
 
 /* digest of one macroblock by one warp: 32 boundary strengths (one lane per edge segment), thresholds of the nine plane x
  * edge-kind combinations.  q, pL, pT: records of the macroblock and of its left and top neighbours in shared memory (pL /
@@ -91,46 +68,6 @@ __device__ __forceinline__ void dbk_digest_mb(const PicJob &J, const E264MbRec *
 	__syncwarp();
 	if (lane < 4) ((uint4 *)(J.dbk + mb))[lane] = ((const uint4 *)dg)[lane];
 	__syncwarp();
-}
-
-/* ---- sample filters on one line across an edge, samples as ints ----
- * Branch-free: a line that is not filtered runs the same arithmetic with its clipping bounds set to zero (a lone
- * warp pays ~10 cycles for every branch it resolves). */
-template <bool STRONG>
-__device__ __forceinline__ void dbk_line_luma(int &p3, int &p2, int &p1, int &p0, int &q0, int &q1, int &q2, int &q3, int bs, int alpha, int beta, int tc0, bool any4) {
-	const int ad = __sad(p0, q0, 0);
-	const bool f = bs != 0 && ad < alpha && __sad(p1, p0, 0) < beta && __sad(q1, q0, 0) < beta;
-	const bool ap = __sad(p2, p0, 0) < beta, aq = __sad(q2, q0, 0) < beta;
-	const int tcp = f && ap ? tc0 : 0, tcq = f && aq ? tc0 : 0;
-	const int tc = f ? tc0 + (int)ap + (int)aq : 0;
-	const int d = min(max((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc), tc);
-	const int avg = (p0 + q0 + 1) >> 1;
-	int n_p1 = p1 + min(max((p2 + avg - (p1 << 1)) >> 1, -tcp), tcp);
-	int n_q1 = q1 + min(max((q2 + avg - (q1 << 1)) >> 1, -tcq), tcq);
-	int n_p0 = mc_clip255(p0 + d), n_q0 = mc_clip255(q0 - d);
-	if (STRONG && any4) {   /* bS 4 exists only on macroblock edges; `any4` is uniform over the warp */
-		const bool s4 = f && bs == 4;
-		const bool small = ad < ((alpha >> 2) + 2);
-		const bool sp = ap && small, sq = aq && small;
-		const int s_p0 = sp ? (p2 + 2 * p1 + 2 * p0 + 2 * q0 + q1 + 4) >> 3 : (2 * p1 + p0 + q1 + 2) >> 2;
-		const int s_p1 = sp ? (p2 + p1 + p0 + q0 + 2) >> 2 : p1;
-		const int s_p2 = sp ? (2 * p3 + 3 * p2 + p1 + p0 + q0 + 4) >> 3 : p2;
-		const int s_q0 = sq ? (p1 + 2 * p0 + 2 * q0 + 2 * q1 + q2 + 4) >> 3 : (2 * q1 + q0 + p1 + 2) >> 2;
-		const int s_q1 = sq ? (p0 + q0 + q1 + q2 + 2) >> 2 : q1;
-		const int s_q2 = sq ? (2 * q3 + 3 * q2 + q1 + q0 + p0 + 4) >> 3 : q2;
-		n_p0 = s4 ? s_p0 : n_p0; n_p1 = s4 ? s_p1 : n_p1; p2 = s4 ? s_p2 : p2;
-		n_q0 = s4 ? s_q0 : n_q0; n_q1 = s4 ? s_q1 : n_q1; q2 = s4 ? s_q2 : q2;
-	}
-	p0 = n_p0; p1 = n_p1; q0 = n_q0; q1 = n_q1;
-}
-__device__ __forceinline__ void dbk_line_chroma(int p1, int &p0, int &q0, int q1, int bs, int alpha, int beta, int tc0) {
-	const bool f = bs != 0 && __sad(p0, q0, 0) < alpha && __sad(p1, p0, 0) < beta && __sad(q1, q0, 0) < beta;
-	const int tc = f ? tc0 + 1 : 0;
-	const int d = min(max((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc), tc);
-	const bool s4 = f && bs == 4;
-	const int n_p0 = s4 ? (2 * p1 + p0 + q1 + 2) >> 2 : mc_clip255(p0 + d);
-	const int n_q0 = s4 ? (2 * q1 + q0 + p1 + 2) >> 2 : mc_clip255(q0 - d);
-	p0 = n_p0; q0 = n_q0;
 }
 
 #define DBK_TS 5      /* tile row stride in words: odd, so the 32 rows of the two halves fall into 32 different banks */

@@ -13,7 +13,12 @@
  * before, so that pictures read slots that pictures in flight still write and overwrite slots they still read.  Extra
  * counters: inflight_max, contexts, ref_slot_in_flight, dst_slot_read_in_flight, and staging_wrapped (pictures submitted
  * while every staging area of the context was in use, so that e264b_acquire_staging had to wait), after one line of
- * pictures per context. */
+ * pictures per context.
+ * --dump DIR (one picture in flight) writes, for every picture of seed k, to DIR/seed_k.bin: its E264PicDesc, records,
+ * slice records, the picture before deblocking and the picture after it (tests/test_deblock_spec.py).  The picture
+ * before deblocking is reconstructed first, from a copy of the records with MBF_DEBLOCK / MBF_EDGE_* cleared and
+ * any_deblock 0, by the port (--cpu-only) or by the device; then the picture is reconstructed as drawn, so the frame
+ * slots hold what they hold without --dump.  The draws are the same with and without it. */
 #define _GNU_SOURCE
 #include <dlfcn.h>
 #include <pthread.h>
@@ -100,7 +105,9 @@ typedef struct {
 	int inflight, n_stage;                 /* pictures submitted ahead at most; staging areas of the device context */
 	Pending *q; int q_head, n_out;         /* the pictures drawn and not yet compared, oldest first */
 	int prev_dst;                          /* slot of the picture drawn last (with pictures in flight) */
+	FILE *dump; E264MbRec *dump_recs; uint8_t *dump_pre, *dump_dev;   /* --dump: the file, flags-cleared records, picture before deblocking */
 } Ctx;
+static const char *dump_dir;
 
 static void geometry(Ctx *c, int W, int H, int n_slots) {
 	memset(&c->g, 0, sizeof(c->g));
@@ -420,12 +427,47 @@ static void dump_mb(const E264MbRec *recs, const E264SliceRec *slices, int W, in
 	        s->wp_mode, s->luma_log2_wd, s->chroma_log2_wd, s->scaling4x4[0][0], s->scaling8x8[0][0]);
 }
 
+/* --dump: one picture's description, records, slices, the picture before deblocking and after it */
+static void dump_picture(Ctx *c, const E264PicDesc *pd, const E264MbRec *recs, const E264SliceRec *slices, const uint8_t *post) {
+	fwrite(pd, sizeof(*pd), 1, c->dump); fwrite(recs, sizeof(E264MbRec), (size_t)c->nmb, c->dump);
+	fwrite(slices, sizeof(E264SliceRec), (size_t)pd->n_slices, c->dump);
+	fwrite(c->dump_pre, 1, (size_t)pd->frame_bytes, c->dump); fwrite(post, 1, (size_t)pd->frame_bytes, c->dump);
+}
+
+/* --dump: the picture before deblocking, reconstructed from the records with the deblocking flags cleared (a picture the
+ * record contract allows), by the port or the device, into c->dump_pre */
+static void reconstruct_pre(Ctx *c, const E264PicDesc *pd, int cpu_only) {
+	E264PicDesc p0 = *pd; p0.any_deblock = 0;
+	memcpy(c->dump_recs, c->recs, (size_t)c->nmb * sizeof(E264MbRec));
+	for (int a = 0; a < c->nmb; a++) c->dump_recs[a].flags &= (uint8_t)~(MBF_DEBLOCK | MBF_EDGE_L | MBF_EDGE_T);
+	if (cpu_only) {
+		pthread_mutex_lock(&port_mu);
+		long res[6], sat = port_cov_wp_bi_sat16;     /* the port's counters count the picture once */
+		memcpy(res, port_cov_residual, sizeof(res));
+		port_recon_picture(c->port_frames, &p0, c->dump_recs, c->coefs, c->slices);
+		memcpy(port_cov_residual, res, sizeof(res)); port_cov_wp_bi_sat16 = sat;
+		pthread_mutex_unlock(&port_mu);
+		memcpy(c->dump_pre, c->port_frames + (size_t)pd->dst_slot * c->g.frame_bytes, (size_t)c->g.frame_bytes);
+		return;
+	}
+	E264Staging st; uint64_t t;
+	if (D.acquire(c->dev, p0.dst_slot, &st)) { fprintf(stderr, "acquire_staging failed\n"); exit(3); }
+	memcpy(st.recs, c->dump_recs, (size_t)c->nmb * sizeof(E264MbRec));
+	memcpy(st.coefs, c->coefs, (size_t)p0.n_coefs * 2);
+	memcpy(st.slices, c->slices, (size_t)p0.n_slices * sizeof(E264SliceRec));
+	memcpy(st.intra_list, c->intra_list, (size_t)p0.n_intra * 4);
+	p0.staging = st.handle;
+	if (D.submit(c->dev, &p0, c->dump_dev, &t) || D.wait(c->dev, t)) { fprintf(stderr, "submit of the picture before deblocking failed\n"); exit(3); }
+	memcpy(c->dump_pre, c->dump_dev, (size_t)c->g.frame_bytes);
+}
+
 /* wait for the oldest picture in flight and compare it with the port's frame of the same picture; returns 0 when they agree */
 static int retire(Ctx *c, int cpu_only) {
 	Pending *p = c->q + c->q_head;
 	c->q_head = (c->q_head + 1) % c->inflight; c->n_out--;
 	if (cpu_only) return 0;
 	if (D.wait(c->dev, p->ticket)) { fprintf(stderr, "picture %d: wait failed\n", p->pic); return 1; }
+	if (c->dump) dump_picture(c, &p->pd, p->recs, p->slices, p->host_out);   /* before the comparison: a picture that fails it is judged too */
 	const int W = c->g.width_mbs, H = c->g.height_mbs;
 	for (int pl = 0; pl < 3; pl++) {
 		int w = pl ? W * 8 : W * 16, h = pl ? H * 8 : H * 16, stride = pl ? c->g.stride_c : c->g.stride_y;
@@ -482,9 +524,11 @@ static int run_picture(Ctx *c, int pic, int dst, int pcm_content, int cpu_only) 
 		for (int k = 0; k < c->n_out; k++) { const Pending *o = c->q + (c->q_head + k) % c->inflight; ref_in |= reads >> o->dst & 1; dst_in |= o->reads >> dst & 1; }
 		cov[C_REF_IN_FLIGHT] += ref_in; cov[C_DST_READ_IN_FLIGHT] += dst_in; cov[C_STAGING_WRAPPED] += c->n_out >= c->n_stage;
 	}
+	if (c->dump) reconstruct_pre(c, &pd, cpu_only);
 	pthread_mutex_lock(&port_mu);
 	port_recon_picture(c->port_frames, &pd, c->recs, c->coefs, c->slices);
 	pthread_mutex_unlock(&port_mu);
+	if (c->dump && cpu_only) dump_picture(c, &pd, c->recs, c->slices, c->port_frames + (size_t)dst * c->g.frame_bytes);
 	Pending *p = c->q + (c->q_head + c->n_out) % c->inflight;
 	p->pic = pic; p->dst = dst; p->reads = reads; p->pd = pd;
 	if (++c->n_out > cov[C_INFLIGHT_MAX]) cov[C_INFLIGHT_MAX] = c->n_out;
@@ -526,6 +570,11 @@ static void *run_context(void *arg) {
 		int n_pics = j->pictures ? j->pictures : W * H >= 4096 ? 3 : W * H >= 100 ? 12 : 24;
 		if (K > 1 && !j->pictures) n_pics += 2 * K;
 		c.q = calloc(K, sizeof(Pending));
+		if (dump_dir) {
+			char path[4096]; snprintf(path, sizeof(path), "%s/seed_%d.bin", dump_dir, seed);
+			if (!(c.dump = fopen(path, "wb"))) { fprintf(stderr, "cannot write %s\n", path); exit(3); }
+			c.dump_recs = malloc((size_t)c.nmb * sizeof(E264MbRec)); c.dump_pre = malloc(c.g.frame_bytes);
+		}
 		if (!cpu_only) {
 			if (D.create(&c.dev)) { fprintf(stderr, "e264b_create failed\n"); exit(3); }
 			if (D.configure(c.dev, &c.g, c.n_slots)) { fprintf(stderr, "e264b_configure failed\n"); exit(3); }
@@ -536,6 +585,7 @@ static void *run_context(void *arg) {
 				p->slices = malloc(MAX_SLICES * sizeof(E264SliceRec)); p->intra_list = malloc((size_t)c.nmb * 4);
 				if (!p->host_out || !p->port || !p->recs || !p->coefs || !p->slices || !p->intra_list) { fprintf(stderr, "out of memory\n"); exit(3); }
 			}
+			if (c.dump) c.dump_dev = D.host_alloc(c.dev, c.g.frame_bytes);
 		}
 		for (int s = 0; s < c.n_slots; s++) {   /* every slot starts identical on both sides */
 			int y = rnd(256), cc = rnd(256);
@@ -552,8 +602,10 @@ static void *run_context(void *arg) {
 		if (bad) { fprintf(stderr, "seed %d (%dx%d, %d slots, pictures %d-%d, %d in flight, %d staging) failed\n", seed, W, H, c.n_slots, first_pic, j->total - 1, K, c.n_stage); j->fails++; }
 		if (!cpu_only) {
 			for (int k = 0; k < K; k++) { Pending *p = c.q + k; D.host_free(c.dev, p->host_out); free(p->port); free(p->recs); free(p->coefs); free(p->slices); free(p->intra_list); }
+			if (c.dump) D.host_free(c.dev, c.dump_dev);
 			D.destroy(c.dev);
 		}
+		if (c.dump) { fclose(c.dump); free(c.dump_recs); free(c.dump_pre); }
 		free(c.q); free(c.port_alloc); free(c.recs); free(c.coefs); free(c.slices); free(c.intra_list);
 	}
 	pthread_mutex_lock(&all.mu);
@@ -575,8 +627,10 @@ int main(int argc, char **argv) {
 		else if (!strcmp(argv[i], "--geom") && i + 1 < argc) sscanf(argv[++i], "%dx%d", &gw, &gh);
 		else if (!strcmp(argv[i], "--contexts") && i + 1 < argc) M = atoi(argv[++i]);
 		else if (!strcmp(argv[i], "--inflight") && i + 1 < argc) K = atoi(argv[++i]);
-		else { fprintf(stderr, "usage: %s [--cpu-only] [--lib path] [--seeds A-B] [--pictures N] [--geom WxH] [--contexts M] [--inflight K]\n", argv[0]); return 2; }
+		else if (!strcmp(argv[i], "--dump") && i + 1 < argc) dump_dir = argv[++i];
+		else { fprintf(stderr, "usage: %s [--cpu-only] [--lib path] [--seeds A-B] [--pictures N] [--geom WxH] [--contexts M] [--inflight K] [--dump DIR]\n", argv[0]); return 2; }
 	}
+	if (dump_dir && K != 1) { fprintf(stderr, "--dump takes one picture in flight\n"); return 2; }
 	if (M < 1 || K < 1 || s1 < s0) { fprintf(stderr, "--contexts and --inflight take at least 1, --seeds A-B needs A <= B\n"); return 2; }
 	if (M > s1 - s0 + 1) M = s1 - s0 + 1;
 	if (!cpu_only) { if (!lib) { fprintf(stderr, "--lib is needed without --cpu-only\n"); return 2; } load_device(lib); }
