@@ -77,6 +77,8 @@ def bind(path):
         lib.edge264_enable_resized.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     if hasattr(lib, "edge264_set_skip"):       # the extension of include/edge264_skip.h
         lib.edge264_set_skip.argtypes = [ctypes.c_void_p, ctypes.c_int]
+    if hasattr(lib, "edge264_enable_luma_only"):   # the extension of include/edge264_luma.h
+        lib.edge264_enable_luma_only.argtypes = [ctypes.c_void_p]
     _loaded[path] = lib
     return lib
 
@@ -155,13 +157,14 @@ def frame_packed(lib, dec, f):
     return out
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None):
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
     carries the frame's motion export (frame_motion); with packed=(format, log2_scale) it ends with the frame's packed
     output (frame_packed); resized=(format, width, height) does the same with the resized output (edge264_enable_resized,
-    log2_scale -1); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip)."""
+    log2_scale -1); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip); luma_only=True decodes
+    the Y plane only, chroma comes out as 128 (edge264_enable_luma_only)."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -194,6 +197,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             d = ctypes.c_void_p(dec)
             lib.edge264_free(ctypes.byref(d))
             raise RuntimeError("edge264_set_skip: %s" % errno.errorcode.get(r, r))
+    if luma_only:
+        r = lib.edge264_enable_luma_only(dec) if hasattr(lib, "edge264_enable_luma_only") else errno.ENOTSUP
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_enable_luma_only: %s" % errno.errorcode.get(r, r))
     nal = base + 3 + (1 if data[2] == 0 else 0)
     frames, codes, f = [], [], Edge264Frame()
     drained = False

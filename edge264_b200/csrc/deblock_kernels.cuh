@@ -35,9 +35,10 @@ struct __align__(16) E264DbkMb {
 };                           /* 64 bytes */
 
 /* digest of one macroblock by one warp: 32 boundary strengths (one lane per edge segment), thresholds of the nine plane x
- * edge-kind combinations.  q, pL, pT: records of the macroblock and of its left and top neighbours in shared memory (pL /
- * pT are read only where the macroblock's flags say that edge is filtered, but must point at readable memory);
- * dg: 64 bytes of shared memory. */
+ * edge-kind combinations (LUMA, luma-only pictures: of the three luma ones; the chroma entries are left unwritten).
+ * q, pL, pT: records of the macroblock and of its left and top neighbours in shared memory (pL / pT are read only where
+ * the macroblock's flags say that edge is filtered, but must point at readable memory); dg: 64 bytes of shared memory. */
+template <bool LUMA>
 __device__ __forceinline__ void dbk_digest_mb(const PicJob &J, const E264MbRec *q, const E264MbRec *pL, const E264MbRec *pT, E264DbkMb *dg, int mb, int lane) {
 	const int qflags = q->flags;
 	const bool on_mb = qflags & MBF_DEBLOCK, fl = qflags & MBF_EDGE_L, ft = qflags & MBF_EDGE_T, t8 = qflags & MBF_T8x8;
@@ -54,7 +55,7 @@ __device__ __forceinline__ void dbk_digest_mb(const PicJob &J, const E264MbRec *
 	unsigned v = (unsigned)bs << ((lane & 7) * 4);
 	v |= __shfl_xor_sync(0xffffffffu, v, 1); v |= __shfl_xor_sync(0xffffffffu, v, 2); v |= __shfl_xor_sync(0xffffffffu, v, 4);
 	if ((lane & 7) == 0) dg->bs[lane >> 3] = v;
-	if (lane < 9) {
+	if (lane < (LUMA ? 3 : 9)) {
 		const int pl = (lane * 11) >> 5, kind = lane - 3 * pl;      /* lane / 3, lane % 3 for lane < 9 */
 		const bool nb = on_mb && (kind == 1 ? fl : kind == 2 && ft);
 		const E264MbRec *p = !nb ? q : kind == 1 ? pL : pT;
@@ -322,23 +323,29 @@ __device__ __forceinline__ void dbk_walk(const PicJob &J, DbkSmem *sm, int band,
 /* MINB blocks per SM = the register budget: the kernel is a chain of dependent steps (a lone warp per scheduler issues
  * about one instruction in five cycles) and holds its registers for the whole picture, so with many pictures in flight
  * the registers of waiting deblocking warps are what the other kernels lack */
-template <int MINB>
+template <int MINB, bool LUMA>
 __global__ void __launch_bounds__(DBK_PAIRS * 32, MINB) e264_deblock_kernel(PicJob J) {
 	TraceScope trace_(J, 3);
 	reset_next_tickets(J);
 	__shared__ DbkSmem sm;
 	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 	const int bands = (J.h_mbs + 2 * DBK_PAIRS - 1) / (2 * DBK_PAIRS);
-	/* bands x {luma, chroma}; tickets in dispatch order: a band only waits for bands drawn before it */
+	/* bands x {luma, chroma} (LUMA, luma-only pictures: bands x luma); tickets in dispatch order: a band only waits for
+	 * bands drawn before it */
 	for (;;) {
 		__syncthreads();
 		if (threadIdx.x < 2 * DBK_PAIRS) { sm.done[threadIdx.x] = 0; sm.taken[threadIdx.x] = 0; }
 		if (threadIdx.x == 0) sm.band = (int)atomicAdd(J.tickets + TICKET_DEBLOCK, 1u);
 		__syncthreads();
 		const int t = sm.band;
-		if (t >= 2 * bands) break;
-		if (t & 1) dbk_walk<true>(J, &sm, t >> 1, wid, lane);
-		else dbk_walk<false>(J, &sm, t >> 1, wid, lane);
+		if (LUMA) {
+			if (t >= bands) break;
+			dbk_walk<false>(J, &sm, t, wid, lane);
+		} else {
+			if (t >= 2 * bands) break;
+			if (t & 1) dbk_walk<true>(J, &sm, t >> 1, wid, lane);
+			else dbk_walk<false>(J, &sm, t >> 1, wid, lane);
+		}
 	}
 }
 

@@ -135,6 +135,7 @@ typedef struct SliceCtx {
 	int error;
 	int missing_ref;          /* a reference-list entry of the slice has no picture (a substitute predicts in its place) */
 	int any_err;              /* a delivered record got a nonzero err (slice_dec.c) */
+	int luma_only;            /* chroma residuals are parsed, then dropped from the pool and the record (edge264_luma.h) */
 	MvCache mc;
 } SliceCtx;
 
@@ -236,6 +237,7 @@ struct Edge264Decoder {
 	int slices_seen;                   /* a slice NAL unit has been decoded (edge264_enable_motion / _packed / _resized are refused from then on) */
 	int packed, packed_format, packed_scale;   /* edge264_enable_packed: every output picture carries its packed output */
 	int packed_width, packed_height;   /* edge264_enable_resized (packed_scale -1): the requested size, one of them possibly 0 */
+	int luma_only;                     /* edge264_enable_luma_only: every picture is reconstructed with luma only */
 	int block_output;                  /* the last decode_NAL asked the application to fetch frames (ENOBUFS, end of stream): get_frame waits for the device */
 	/* scratch: RBSP of the last non-slice NAL unit */
 	uint8_t *rbsp; size_t rbsp_cap;

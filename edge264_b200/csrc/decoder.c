@@ -18,6 +18,7 @@
 #include "../../include/edge264_motion.h"
 #include "../../include/edge264_packed.h"
 #include "../../include/edge264_skip.h"
+#include "../../include/edge264_luma.h"
 
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
@@ -410,6 +411,7 @@ static void build_finalize(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd) {
 	pd->width_mbs = d->w_mbs; pd->height_mbs = d->h_mbs; pd->stride_y = d->stride_y; pd->stride_c = d->stride_c;
 	pd->plane_y = d->plane_y; pd->frame_bytes = d->frame_bytes; pd->dst_slot = pb->slot;
 	pd->n_slices = pb->n_slices; pd->n_coefs = (int32_t)pb->n_coefs; pd->any_deblock = pb->any_deblock; pd->staging = pb->staging;
+	pd->luma_only = (uint8_t)d->luma_only;
 	/* intra macroblocks in raster order: the device draws them from this list, so a waiting macroblock only ever waits for earlier entries */
 	const int total = d->w_mbs * d->h_mbs; int n = 0;
 	for (int a = 0; a < total; a++) if (pb->recs[a].kind != MBK_INTER) pb->intra_list[n++] = (uint32_t)a;
@@ -943,7 +945,7 @@ static int fill_frame_num_gap(Edge264Decoder *d, int frame_num_abs) {
 		}
 		np->poc = np->poc_dec = np->poc_top = np->poc_top_dec = npoc;
 		for (int i = 0; i < E264_MAX_SLOTS; i++) np->slot_uid[i] = -1;
-		if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, 0); pthread_mutex_unlock(&d->be_lock); }
+		if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, d->luma_only ? 128 : 0); pthread_mutex_unlock(&d->be_lock); }
 		d->taint |= 1u << sl;   /* its error map is all 100 */
 	}
 	d->prev_ref_frame_num = frame_num_abs - 1;   /* the last inserted frame is the previous reference frame now (headers.c:1131) */
@@ -1080,7 +1082,7 @@ static void fill_skipped(Edge264Decoder *d, int slot) {
 	if (!d->pics[slot].unfilled) return;
 	d->pics[slot].unfilled = 0;
 	threads_drain(d, d->pb);
-	if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, slot, 0, 0); pthread_mutex_unlock(&d->be_lock); }
+	if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, slot, 0, d->luma_only ? 128 : 0); pthread_mutex_unlock(&d->be_lock); }
 	d->taint |= 1u << slot;
 }
 
@@ -1108,7 +1110,7 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 	c->qp = h->slice_qp; c->chroma_qp_offset[0] = p->chroma_qp_index_offset[0]; c->chroma_qp_offset[1] = p->chroma_qp_index_offset[1];
 	c->deblock_idc = h->deblock_idc; c->cur_poc = cp->poc_dec;
 	c->mbi = pb->mbi; c->recs = pb->recs; c->coefs = pb->coefs; c->coef_cap = pb->coef_cap;   /* n_coefs: build_work continues the pool where the previous slice ended */
-	c->col_recs = NULL; c->col_slot_uid = NULL; c->error = 0; c->n_intra = 0; c->missing_ref = 0; c->any_err = 0;
+	c->col_recs = NULL; c->col_slot_uid = NULL; c->error = 0; c->n_intra = 0; c->missing_ref = 0; c->any_err = 0; c->luma_only = d->luma_only;
 	memset(c->ref_slot, -1, sizeof(c->ref_slot)); memset(c->ref_long, 0, sizeof(c->ref_long));
 	for (int l = 0; l < 2; l++) for (int i = 0; i < 32; i++) { c->ref_uid[l][i] = -1; c->ref_poc[l][i] = 0; }
 	if (h->slice_type < 2) {
@@ -1140,6 +1142,10 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 		int wp = h->slice_type == 0 ? p->weighted_pred_flag : p->weighted_bipred_idc;
 		sr->wp_mode = (uint8_t)wp; sr->luma_log2_wd = (uint8_t)h->luma_log2_wd; sr->chroma_log2_wd = (uint8_t)h->chroma_log2_wd;
 		if (wp == 1) for (int l = 0; l < 2; l++) for (int i = 0; i < 16; i++) for (int k = 0; k < 3; k++) { sr->wp_w[l][i][k] = h->w[l][i][k]; sr->wp_o[l][i][k] = h->o[l][i][k]; }
+		if (wp == 1 && d->luma_only) {   /* chroma weights that keep 128 at 128 (edge264_enable_luma_only) */
+			sr->chroma_log2_wd = 0;
+			for (int l = 0; l < 2; l++) for (int i = 0; i < 16; i++) for (int k = 1; k < 3; k++) { sr->wp_w[l][i][k] = 1; sr->wp_o[l][i][k] = 0; }
+		}
 		if (wp == 2) implicit_weights(c, sr);
 	}
 	pb->n_slices++;
@@ -1409,5 +1415,20 @@ int edge264_get_packed(Edge264Decoder *d, const Edge264Frame *frame, Edge264Pack
 int edge264_set_skip(Edge264Decoder *d, int mode) {
 	if (!d || mode < EDGE264_SKIP_NONE || mode > EDGE264_SKIP_NONKEY) return EINVAL;
 	d->skip_mode = mode;   /* read by start_picture only: the current picture keeps its decision */
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* luma-only decoding (include/edge264_luma.h)                                                  */
+/* ------------------------------------------------------------------------------------------ */
+/* The records of a luma-only picture reconstruct a chroma plane of 128 on their own, whatever backend reconstructs them:
+ * no chroma levels (sx_residual), chroma samples of I_PCM macroblocks set to 128 (mb_impl.h), explicit chroma weights 1 with
+ * offset 0 and log2 denominator 0 (setup_slice), filled slots at 128 (fill_slot).  With every reference at 128, intra
+ * prediction of every mode, interpolation, every weighting and the deblocking filter map a plane of 128 to itself.  The
+ * device's luma-only kernels leave chroma alone and set it to 128 with a memset: both give the same frame. */
+int edge264_enable_luma_only(Edge264Decoder *d) {
+	if (!d) return EINVAL;
+	if (d->slices_seen) return EBUSY;   /* the pictures of one stream are all decoded one way */
+	d->luma_only = 1;
 	return 0;
 }

@@ -96,6 +96,7 @@ struct __align__(16) InterSmem {
  * used to carry their own copies: 3 000 of the kernel's 12 000 instructions, and with blocks of several pictures in
  * different phases on an SM the instruction cache, 32 KB in its first shared level, is what the warps wait for);
  * `cls` is uniform over the warp, so the switch is one resolved branch per pass. */
+template <bool LUMA>   /* luma-only pictures: no chroma windows, no chroma predictions */
 __device__ __forceinline__ void inter_item(const PicJob &J, InterSmem &sm, int cls, int item, int mb0, int W, int H) {
 	const int m = item >> 5, l = (item >> 4) & 1, z = item & 15, bx = blk_x(z), by = blk_y(z);
 	const E264MbRec *r = (const E264MbRec *)sm.rec4[m];
@@ -108,10 +109,12 @@ __device__ __forceinline__ void inter_item(const PicJob &J, InterSmem &sm, int c
 	uint32_t win[9][3], py[4];
 	mc_load_luma(ref, J.stride_y, W, H, mbx * 16 + bx * 4 + (mvx >> 2) - 2, mby * 16 + by * 4 + (mvy >> 2) - 2, win);
 	uint32_t cb[3], cr[3];
-	const uint8_t *cplane = ref + J.plane_y;
-	const int cx = mbx * 8 + bx * 2 + (mvx >> 3), cy = mby * 8 + by * 2 + (mvy >> 3);
-	mc_load_chroma(cplane, J.stride_c, W >> 1, H >> 1, cx, cy, cb);
-	mc_load_chroma(cplane + (J.stride_c >> 1), J.stride_c, W >> 1, H >> 1, cx, cy, cr);
+	if (!LUMA) {
+		const uint8_t *cplane = ref + J.plane_y;
+		const int cx = mbx * 8 + bx * 2 + (mvx >> 3), cy = mby * 8 + by * 2 + (mvy >> 3);
+		mc_load_chroma(cplane, J.stride_c, W >> 1, H >> 1, cx, cy, cb);
+		mc_load_chroma(cplane + (J.stride_c >> 1), J.stride_c, W >> 1, H >> 1, cx, cy, cr);
+	}
 	switch (cls) {
 	case 0:
 #pragma unroll
@@ -125,10 +128,11 @@ __device__ __forceinline__ void inter_item(const PicJob &J, InterSmem &sm, int c
 	}
 	uint32_t *o = sm.pred[m][l][z];
 	*(uint4 *)o = make_uint4(py[0], py[1], py[2], py[3]);
-	*(uint2 *)(o + 4) = make_uint2(mc_chroma2x2(cb[0], cb[1], cb[2], mvx & 7, mvy & 7), mc_chroma2x2(cr[0], cr[1], cr[2], mvx & 7, mvy & 7));
+	if (!LUMA) *(uint2 *)(o + 4) = make_uint2(mc_chroma2x2(cb[0], cb[1], cb[2], mvx & 7, mvy & 7), mc_chroma2x2(cr[0], cr[1], cr[2], mvx & 7, mvy & 7));
 }
 
-template <int MINB>
+/* LUMA: luma-only pictures (PicDesc.luma_only), which neither read nor write a chroma sample */
+template <int MINB, bool LUMA>
 __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(PicJob J) {
 	TraceScope trace_(J, 1);
 	reset_next_tickets(J);
@@ -197,7 +201,7 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 #pragma unroll
 				for (int j = 0; j < 6; j++) { const int gj = (sm.qn[j] + 31) >> 5; if (g >= acc) { c = j; gb = acc; } acc += gj; }
 				const int k = (g - gb) * 32 + lane;
-				if (k < sm.qn[c]) inter_item(J, sm, c, sm.queue[c][k], mb0, W, H);
+				if (k < sm.qn[c]) inter_item<LUMA>(J, sm, c, sm.queue[c][k], mb0, W, H);
 			}
 		}
 		PT_MARK(1)      /* prediction passes */
@@ -212,7 +216,7 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 			/* the macroblock's deblocking digest (every macroblock, intra ones too), from the records in shared memory, while
 			 * the coefficient run requested above is in flight */
 			if (J.dbk != nullptr)
-				dbk_digest_mb(J, (const E264MbRec *)sm.rec4[m], (const E264MbRec *)(m > 0 ? sm.rec4[m - 1] : sm.lrec4), (const E264MbRec *)sm.trec4[m], &sm.ddg[w], mb0 + m, lane);
+				dbk_digest_mb<LUMA>(J, (const E264MbRec *)sm.rec4[m], (const E264MbRec *)(m > 0 ? sm.rec4[m - 1] : sm.lrec4), (const E264MbRec *)sm.trec4[m], &sm.ddg[w], mb0 + m, lane);
 			PT_MARK(3)          /* deblocking digest */
 			if (what) {
 				const int mb = mb0 + m, mbx = mb % J.w_mbs, mby = mb / J.w_mbs;
@@ -222,7 +226,7 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 					if (!mbar_wait(&sm.bars[w][b], parity[b])) { if (lane == 0) atomicExch(J.err, 4u); failed = true; }
 					parity[b] ^= 1;
 					PT_MARK(4)  /* waiting for the coefficient run */
-					if (!failed) residual_stage(ws, r, sr, sm.coef[w][b], lane);
+					if (!failed) residual_stage<LUMA>(ws, r, sr, sm.coef[w][b], lane);
 					PT_MARK(5)  /* dequantisation and inverse transforms */
 				}
 				if (!failed) {
@@ -231,40 +235,40 @@ __global__ void __launch_bounds__(INTER_WARPS * 32, MINB) e264_inter4_kernel(Pic
 					const int z = lane & 15, h = lane >> 4, bx = blk_x(z), by = blk_y(z), i8 = z >> 2;
 					const int r0 = r->ref_idx[0][i8], r1 = r->ref_idx[1][i8];
 					uint32_t py[2] = {0, 0}, pc = 0, qy[2] = {0, 0}, qc = 0;
-					if (r0 >= 0) { const uint2 a = *(const uint2 *)(sm.pred[m][0][z] + 2 * h); py[0] = a.x; py[1] = a.y; pc = sm.pred[m][0][z][4 + h]; }
-					if (r1 >= 0) { const uint2 a = *(const uint2 *)(sm.pred[m][1][z] + 2 * h); qy[0] = a.x; qy[1] = a.y; qc = sm.pred[m][1][z][4 + h]; }
+					if (r0 >= 0) { const uint2 a = *(const uint2 *)(sm.pred[m][0][z] + 2 * h); py[0] = a.x; py[1] = a.y; if (!LUMA) pc = sm.pred[m][0][z][4 + h]; }
+					if (r1 >= 0) { const uint2 a = *(const uint2 *)(sm.pred[m][1][z] + 2 * h); qy[0] = a.x; qy[1] = a.y; if (!LUMA) qc = sm.pred[m][1][z][4 + h]; }
 					const int wpm = sr->wp_mode;
 					const bool bi = r0 >= 0 && r1 >= 0;
 					if (!bi && r0 < 0) { py[0] = qy[0]; py[1] = qy[1]; pc = qc; }
 					if (bi && wpm == WP_DEFAULT) {
-						py[0] = mc_avg4(py[0], qy[0]); py[1] = mc_avg4(py[1], qy[1]); pc = mc_avg4(pc, qc);
+						py[0] = mc_avg4(py[0], qy[0]); py[1] = mc_avg4(py[1], qy[1]); if (!LUMA) pc = mc_avg4(pc, qc);
 					} else if ((bi && wpm != WP_DEFAULT) || (wpm == WP_EXPLICIT && (r0 >= 0 || r1 >= 0))) {
 						/* one weighting body for every scheme: parameters of luma and of this lane's chroma plane, then three words */
 						int wa[2], wb[2], o[2], sh[2], rnd[2];
 						const int ll = r0 >= 0 ? 0 : 1, ri = (ll ? r1 : r0) & 15;
 #pragma unroll
-						for (int k = 0; k < 2; k++) {
+						for (int k = 0; k < (LUMA ? 1 : 2); k++) {
 							const int c = k ? 1 + h : 0, lw = k ? sr->chroma_log2_wd : sr->luma_log2_wd;
 							if (bi && wpm == WP_EXPLICIT) { wa[k] = sr->wp_w[0][r0 & 15][c]; wb[k] = sr->wp_w[1][r1 & 15][c]; o[k] = 0; sh[k] = lw + 1; rnd[k] = ((sr->wp_o[0][r0 & 15][c] + sr->wp_o[1][r1 & 15][c] + 1) | 1) * (1 << lw); }
 							else if (bi) { wb[k] = sr->implicit_w1[r0 & 15][r1 & 15]; wa[k] = 64 - wb[k]; o[k] = 0; sh[k] = 6; rnd[k] = 32; }
 							else { wa[k] = sr->wp_w[ll][ri][c]; wb[k] = 0; o[k] = sr->wp_o[ll][ri][c]; sh[k] = lw; rnd[k] = lw >= 1 ? 1 << (lw - 1) : 0; }
 						}
 						py[0] = wp_word(py[0], qy[0], wa[0], wb[0], rnd[0], sh[0], o[0]); py[1] = wp_word(py[1], qy[1], wa[0], wb[0], rnd[0], sh[0], o[0]);
-						pc = wp_word(pc, qc, wa[1], wb[1], rnd[1], sh[1], o[1]);
+						if (!LUMA) pc = wp_word(pc, qc, wa[1], wb[1], rnd[1], sh[1], o[1]);
 					}
 					if (what == 2) {
 						const int16_t *ry = ws->res + (by * 4 + 2 * h) * 16 + bx * 4, *rc = ws->res + 256 + h * 64 + (by * 2) * 8 + bx * 2;
 						const uint2 res0 = *(const uint2 *)ry, res1 = *(const uint2 *)(ry + 16);
 						py[0] = mc_add_res4(py[0], res0.x, res0.y); py[1] = mc_add_res4(py[1], res1.x, res1.y);
-						pc = mc_add_res4(pc, *(const uint32_t *)rc, *(const uint32_t *)(rc + 8));
+						if (!LUMA) pc = mc_add_res4(pc, *(const uint32_t *)rc, *(const uint32_t *)(rc + 8));
 					}
 					*(uint32_t *)&YT(bx * 4, by * 4 + 2 * h) = py[0]; *(uint32_t *)&YT(bx * 4, by * 4 + 2 * h + 1) = py[1];
-					*(uint16_t *)&CT(h, bx * 2, by * 2) = (uint16_t)pc; *(uint16_t *)&CT(h, bx * 2, by * 2 + 1) = (uint16_t)(pc >> 16);
+					if (!LUMA) { *(uint16_t *)&CT(h, bx * 2, by * 2) = (uint16_t)pc; *(uint16_t *)&CT(h, bx * 2, by * 2 + 1) = (uint16_t)(pc >> 16); }
 				}
 				__syncwarp();
 				if (!failed) {
 					uint8_t *Y, *C; mb_planes(J, mbx, mby, Y, C);
-					store_mb(ws, J, Y, C, lane);
+					store_mb<LUMA>(ws, J, Y, C, lane);
 					if (lane == 0) J.flags[mb] = J.epoch;     /* visible to the intra kernel through the kernel boundary */
 				}
 				__syncwarp();

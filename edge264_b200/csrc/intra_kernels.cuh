@@ -42,6 +42,7 @@ struct __align__(16) IntraRowsSmem {
  * dequantisation and inverse transforms into the residual of slot x % IR_SLOTS, at most IR_SLOTS - 1 macroblocks ahead of
  * the prediction warp.  In a picture without inter macroblocks it also derives the row's deblocking digests (no inter
  * kernel runs that would). */
+template <bool LUMA>
 __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSmem &sm, int band, int w, int lane, unsigned &parbits) {
 	const int W = J.w_mbs, H = J.h_mbs, nmb = W * H;
 	const int mby = band * IR_ROWS + w;
@@ -93,7 +94,7 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 			if (!mbar_wait(&sm.bars[w][sl], (parbits >> sl) & 1)) { if (lane == 0) atomicExch(J.err, 3u); }
 			parbits ^= 1u << sl;
 			PT_MARK(2)  /* waiting for the coefficient run */
-			residual_stage(ws, r, J.slices + r->slice_idx, sm.coef[w][sl], lane);
+			residual_stage<LUMA>(ws, r, J.slices + r->slice_idx, sm.coef[w][sl], lane);
 		} else if (kind != MBK_INTER && kind != MBK_IPCM) clear_residual(ws, lane);
 		__syncwarp();
 		if (lane == 0) { __threadfence_block(); *ready = mbx + 1; }
@@ -102,7 +103,7 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 			if (lane < 12) sm.drecs[w][lane] = topreg;
 			if (mby > 0 && mbx + 1 < W && lane < 12) topreg = __ldg((const uint4 *)(rowrecs - W + mbx + 1) + lane);
 			__syncwarp();
-			dbk_digest_mb(J, r, (const E264MbRec *)sm.recs[w][(mbx + IR_RECS - 1) % IR_RECS], (const E264MbRec *)sm.drecs[w], &sm.ddg[w], mby * W + mbx, lane);
+			dbk_digest_mb<LUMA>(J, r, (const E264MbRec *)sm.recs[w][(mbx + IR_RECS - 1) % IR_RECS], (const E264MbRec *)sm.drecs[w], &sm.ddg[w], mby * W + mbx, lane);
 		}
 		PT_MARK(4)      /* deblocking digest */
 	}
@@ -110,8 +111,9 @@ __device__ __forceinline__ void intra_row_transform(const PicJob &J, IntraRowsSm
 }
 
 /* The row's PREDICTION warp: waits for the residual, for the row above (top-right neighbour finished) and for room in
- * its ring, predicts into the tile of slot x % IR_SLOTS, stores, hands the bottom sample row down. */
-template <bool MAPS>
+ * its ring, predicts into the tile of slot x % IR_SLOTS, stores, hands the bottom sample row down.  LUMA: luma-only
+ * pictures, no chroma sample is read, predicted, stored or handed over. */
+template <bool MAPS, bool LUMA>
 __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &sm, int band, int w, int lane) {
 	const int W = J.w_mbs, H = J.h_mbs;
 	const int lrow = w, mby = band * IR_ROWS + w;
@@ -159,32 +161,32 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 			if (lane < 4) *(uint32_t *)&YT(4 * lane, -1) = ring_in[mbx % IR_RING][lane];
 			else if (lane < 6) { if (mbx + 1 < W) *(uint32_t *)&YT(16 + 4 * (lane - 4), -1) = ring_in[(mbx + 1) % IR_RING][lane - 4]; }
 			else if (lane == 6) { if (mbx > 0) YT(-1, -1) = (uint8_t)(ring_in[(mbx - 1) % IR_RING][3] >> 24); }
-			else if (lane >= 8 && lane < 12) *(uint32_t *)&CT((lane - 8) >> 1, 4 * (lane & 1), -1) = ring_in[mbx % IR_RING][lane - 4];
-			else if (lane == 12) { if (mbx > 0) CT(0, -1, -1) = (uint8_t)(ring_in[(mbx - 1) % IR_RING][5] >> 24); }
-			else if (lane == 13) { if (mbx > 0) CT(1, -1, -1) = (uint8_t)(ring_in[(mbx - 1) % IR_RING][7] >> 24); }
-		} else if (from_global) load_row_above(ws, Y - J.stride_y, C - J.stride_c, cpl, mbx > 0, mbx < W - 1, lane);
+			else if (!LUMA && lane >= 8 && lane < 12) *(uint32_t *)&CT((lane - 8) >> 1, 4 * (lane & 1), -1) = ring_in[mbx % IR_RING][lane - 4];
+			else if (!LUMA && lane == 12) { if (mbx > 0) CT(0, -1, -1) = (uint8_t)(ring_in[(mbx - 1) % IR_RING][5] >> 24); }
+			else if (!LUMA && lane == 13) { if (mbx > 0) CT(1, -1, -1) = (uint8_t)(ring_in[(mbx - 1) % IR_RING][7] >> 24); }
+		} else if (from_global) load_row_above<LUMA>(ws, Y - J.stride_y, C - J.stride_c, cpl, mbx > 0, mbx < W - 1, lane);
 		__syncwarp();
 		PT_MARK(2)      /* ring room, hand-shake, row above into the tile */
 		/* ---- the macroblock ---- */
 		if (kind == MBK_INTER) {   /* reconstructed by the inter kernel: fetch its right column and bottom row for the neighbours to come */
 			if (lane < 16) YT(15, lane) = __ldcg(Y + (size_t)lane * J.stride_y + 15);
-			else { const int j = lane - 16; CT(j >> 3, 7, j & 7) = __ldcg(C + (j >> 3) * cpl + (size_t)(j & 7) * J.stride_c + 7); }
+			else if (!LUMA) { const int j = lane - 16; CT(j >> 3, 7, j & 7) = __ldcg(C + (j >> 3) * cpl + (size_t)(j & 7) * J.stride_c + 7); }
 			if (to_ring) {
 				if (lane < 4) ring_out[mbx % IR_RING][lane] = __ldcg((const uint32_t *)(Y + (size_t)15 * J.stride_y) + lane);
-				else if (lane < 8) ring_out[mbx % IR_RING][lane] = __ldcg((const uint32_t *)(C + ((lane - 4) >> 1) * cpl + (size_t)7 * J.stride_c) + (lane & 1));
+				else if (!LUMA && lane < 8) ring_out[mbx % IR_RING][lane] = __ldcg((const uint32_t *)(C + ((lane - 4) >> 1) * cpl + (size_t)7 * J.stride_c) + (lane & 1));
 			}
 		} else {
-			if (kind == MBK_IPCM) load_pcm(ws, J, r, lane);
+			if (kind == MBK_IPCM) load_pcm<LUMA>(ws, J, r, lane);
 			else {
 				intra_luma(ws, r, lane);
 				PT_MARK(3)  /* luma prediction */
-				intra_chroma(ws, r, lane);
+				if (!LUMA) intra_chroma(ws, r, lane);
 				PT_MARK(4)  /* chroma prediction */
 			}
-			store_mb(ws, J, Y, C, lane);
+			store_mb<LUMA>(ws, J, Y, C, lane);
 			if (to_ring) {
 				if (lane < 4) ring_out[mbx % IR_RING][lane] = *(const uint32_t *)&YT(4 * lane, 15);
-				else if (lane < 8) ring_out[mbx % IR_RING][lane] = *(const uint32_t *)&CT((lane - 4) >> 1, 4 * (lane & 1), 7);
+				else if (!LUMA && lane < 8) ring_out[mbx % IR_RING][lane] = *(const uint32_t *)&CT((lane - 4) >> 1, 4 * (lane & 1), 7);
 			}
 		}
 		__syncwarp();
@@ -215,8 +217,8 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 		{
 			WarpSmem *wn = &sm.ws[w][(mbx + 1) % IR_SLOTS];
 			if (lane < 16) wn->ytile[(lane + 1) * YT_STRIDE + 15] = YT(15, lane);
-			else if (lane < 24) wn->ctile[0][(lane - 16 + 1) * CT_STRIDE + 7] = CT(0, 7, lane - 16);
-			if (lane < 8) wn->ctile[1][(lane + 1) * CT_STRIDE + 7] = CT(1, 7, lane);
+			else if (!LUMA && lane < 24) wn->ctile[0][(lane - 16 + 1) * CT_STRIDE + 7] = CT(0, 7, lane - 16);
+			if (!LUMA && lane < 8) wn->ctile[1][(lane + 1) * CT_STRIDE + 7] = CT(1, 7, lane);
 		}
 		__syncwarp();
 		if (lane == 0) { __threadfence_block(); *used = mbx + 1; }
@@ -231,10 +233,12 @@ __device__ __forceinline__ void intra_row_walk(const PicJob &J, IntraRowsSmem &s
 	}
 }
 
-/* MAPS: the picture has err_pic (recon.cu launches the instantiation that matches it, so clean pictures run code without
- * any map work) */
-template <bool MAPS>
-__global__ void __launch_bounds__(IR_ROWS * 64) e264_intra_rows_kernel(PicJob J) {
+/* MAPS: the picture has err_pic; LUMA: the picture is luma-only (recon.cu launches the instantiation that matches them,
+ * so clean colour pictures run code without any map or luma-only test).  The luma-only instantiations state one block
+ * per SM: without it ptxas fits them into 64 registers and spills (with it 104 / 106, no spill); 0 leaves the colour
+ * ones as they were */
+template <bool MAPS, bool LUMA>
+__global__ void __launch_bounds__(IR_ROWS * 64, LUMA ? 1 : 0) e264_intra_rows_kernel(PicJob J) {
 	TraceScope trace_(J, 2);
 	reset_next_tickets(J);
 	extern __shared__ __align__(16) unsigned char ir_smem_raw[];
@@ -252,8 +256,8 @@ __global__ void __launch_bounds__(IR_ROWS * 64) e264_intra_rows_kernel(PicJob J)
 		__syncthreads();
 		const int band = sm.band;
 		if (band >= bands) break;
-		if (transform) intra_row_transform(J, sm, band, w, lane, parbits);
-		else intra_row_walk<MAPS>(J, sm, band, w, lane);
+		if (transform) intra_row_transform<LUMA>(J, sm, band, w, lane, parbits);
+		else intra_row_walk<MAPS, LUMA>(J, sm, band, w, lane);
 	}
 }
 
@@ -287,7 +291,7 @@ __device__ __noinline__ void intra_error_byte(uint8_t *map, const E264MbRec *r, 
 	const unsigned e = __reduce_max_sync(0xffffffffu, idx >= 0 ? (unsigned)__ldcg(map + idx) : 0u);
 	if (lane == 0) map[mb] = (uint8_t)max(e, (unsigned)r->err);
 }
-template <bool MAPS>   /* as for e264_intra_rows_kernel */
+template <bool MAPS, bool LUMA>   /* as for e264_intra_rows_kernel */
 __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) {
 	TraceScope trace_(J, 2);
 	reset_next_tickets(J);
@@ -314,14 +318,14 @@ __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) 
 		if (kind == MBK_INTER) continue;      /* (the list holds intra macroblocks only) */
 		uint8_t *Y, *C; mb_planes(J, mbx, mby, Y, C);
 		if (kind == MBK_IPCM) {
-			load_pcm(ws, J, r, lane);
-			store_mb(ws, J, Y, C, lane);
+			load_pcm<LUMA>(ws, J, r, lane);
+			store_mb<LUMA>(ws, J, Y, C, lane);
 		} else {
 			if (r->coded != 0) {
 				coef_request(J, r, sm.coef[w], &sm.bars[w], lane);
 				if (!mbar_wait(&sm.bars[w], parity)) { if (lane == 0) atomicExch(J.err, 3u); }
 				parity ^= 1;
-				residual_stage(ws, r, J.slices + r->slice_idx, sm.coef[w], lane);
+				residual_stage<LUMA>(ws, r, J.slices + r->slice_idx, sm.coef[w], lane);
 			} else clear_residual(ws, lane);
 			{	/* A, D, B, C: one lane each, the four round trips overlap */
 				int idx = -1;
@@ -332,15 +336,15 @@ __global__ void __launch_bounds__(INTRA_WARPS * 32) e264_intra_kernel(PicJob J) 
 				if (idx >= 0) wait_flag_acquire(J.flags, idx, J.epoch, J.err);
 			}
 			__syncwarp();
-			if (mby > 0) load_row_above(ws, Y - J.stride_y, C - J.stride_c, cpl, mbx > 0, mbx < W - 1, lane);
+			if (mby > 0) load_row_above<LUMA>(ws, Y - J.stride_y, C - J.stride_c, cpl, mbx > 0, mbx < W - 1, lane);
 			if (mbx > 0) {
 				if (lane < 16) YT(-1, lane) = __ldcg(Y + (size_t)lane * J.stride_y - 1);
-				else { const int j = lane - 16, pl = j >> 3, row = j & 7; CT(pl, -1, row) = __ldcg(C + pl * cpl + (size_t)row * J.stride_c - 1); }
+				else if (!LUMA) { const int j = lane - 16, pl = j >> 3, row = j & 7; CT(pl, -1, row) = __ldcg(C + pl * cpl + (size_t)row * J.stride_c - 1); }
 			}
 			__syncwarp();
 			intra_luma(ws, r, lane);
-			intra_chroma(ws, r, lane);
-			store_mb(ws, J, Y, C, lane);
+			if (!LUMA) intra_chroma(ws, r, lane);
+			store_mb<LUMA>(ws, J, Y, C, lane);
 		}
 		__syncwarp();
 		if (MAPS) intra_error_byte(map_of(J, J.dst_slot), r, mb, W, lane);   /* before the flag: the macroblocks that wait for it read the byte */

@@ -333,6 +333,7 @@ static void sx_macroblock(SliceCtx *s) {
 				memcpy(dst, s->br.buf + (s->br.pos >> 3), 384);
 				s->br.pos += 384 * 8;
 			}
+			if (s->luma_only) memset((uint8_t *)dst + 256, 128, 128);   /* luma only: the chroma samples are 128 (edge264_luma.h) */
 #endif
 			m->cbp = 0x2f; m->cbf_dc = 7; m->cbf_luma = 0xffff; m->cbf_cb = m->cbf_cr = 15;
 			memset(m->tc, 16, 24);

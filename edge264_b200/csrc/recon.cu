@@ -94,6 +94,20 @@ static void free_geometry(E264bDevice *c) {
 	c->kept.clear();
 }
 
+/* the dynamic shared memory of the kernels that take more than the default, for colour (LUMA false) and luma-only pictures */
+template <bool LUMA> static int set_smem_limits() {
+	CK(cudaFuncSetAttribute(e264_intra_rows_kernel<false, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraRowsSmem)));
+	CK(cudaFuncSetAttribute(e264_intra_rows_kernel<true, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraRowsSmem)));
+	CK(cudaFuncSetAttribute(e264_inter4_kernel<INTER_MINB0, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
+	CK(cudaFuncSetAttribute(e264_intra_kernel<false, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraTkSmem)));
+	CK(cudaFuncSetAttribute(e264_intra_kernel<true, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraTkSmem)));
+#if INTER_WARPS == 4
+	CK(cudaFuncSetAttribute(e264_inter4_kernel<6, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
+	CK(cudaFuncSetAttribute(e264_inter4_kernel<8, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
+#endif
+	return 0;
+}
+
 extern "C" int e264b_create(E264bDevice **out) {
 	int n = 0;
 	if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
@@ -118,15 +132,7 @@ extern "C" int e264b_create(E264bDevice **out) {
 	memset(c->h_recs, 0, sizeof(c->h_recs)); memset(c->rec_busy, 0, sizeof(c->rec_busy)); memset(c->st, 0, sizeof(c->st)); c->stage = 0; c->d_sync = NULL; c->epoch = 0; c->tick_seq = 0;
 	c->launches = c->h2d_bytes = c->d2h_bytes = 0;
 	c->dev = dev;
-	CK(cudaFuncSetAttribute(e264_intra_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraRowsSmem)));
-	CK(cudaFuncSetAttribute(e264_intra_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraRowsSmem)));
-	CK(cudaFuncSetAttribute(e264_inter4_kernel<INTER_MINB0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
-	CK(cudaFuncSetAttribute(e264_intra_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraTkSmem)));
-	CK(cudaFuncSetAttribute(e264_intra_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IntraTkSmem)));
-#if INTER_WARPS == 4
-	CK(cudaFuncSetAttribute(e264_inter4_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
-	CK(cudaFuncSetAttribute(e264_inter4_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InterSmem)));
-#endif
+	if (set_smem_limits<false>() || set_smem_limits<true>()) return -1;
 	CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
 	for (int i = 0; i < E264_MAX_SLOTS; i++) CK(cudaEventCreateWithFlags(&c->rec_up[i], cudaEventDisableTiming | cudaEventBlockingSync));
 	for (int i = 0; i < NSTAGE; i++) CK(cudaEventCreateWithFlags(&c->st[i].done, cudaEventDisableTiming | cudaEventBlockingSync));
@@ -264,7 +270,8 @@ static PicJob make_job(E264bDevice *c, const E264PicDesc *pd, int stage, const E
 	J.tickets = c->d_sync + SYNC_TICKETS + (J.epoch & 1) * 4; J.tickets_next = c->d_sync + SYNC_TICKETS + ((J.epoch + 1) & 1) * 4;    /* two sets, pictures alternate; every kernel clears the next picture's */
 	return J;
 }
-static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd, int with_deblock) {
+/* the kernels of one picture; LUMA: the luma-only instantiations (pd->luma_only) */
+template <bool LUMA> static int launch_kernels(E264bDevice *c, const PicJob &J, const E264PicDesc *pd, int with_deblock) {
 	const int nmb = J.w_mbs * J.h_mbs;
 	const int cap = c->sm_count * 8;
 	static int minb = -1, dm = -1;
@@ -276,7 +283,7 @@ static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd
 	if (only < 0) { const char *e = getenv("E264B_REPLAY_ONLY"); only = e && atoi(e) > 0 ? atoi(e) : 7; }
 	if (dbk_smem < 0) {
 		const char *e = getenv("E264B_DBK_SMEM"); dbk_smem = e ? atoi(e) : 0;
-		if (dbk_smem > 0) { cudaFuncSetAttribute(e264_deblock_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, dbk_smem); cudaFuncSetAttribute(e264_deblock_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, dbk_smem); cudaFuncSetAttribute(e264_deblock_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, dbk_smem); }
+		if (dbk_smem > 0) { cudaFuncSetAttribute(e264_deblock_kernel<2, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, dbk_smem); cudaFuncSetAttribute(e264_deblock_kernel<4, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, dbk_smem); cudaFuncSetAttribute(e264_deblock_kernel<5, LUMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, dbk_smem); }
 	}
 	const int mask = J.trace ? only : 7;
 	/* up to three launches per picture, nothing in between: inter macroblocks (inverse transform + prediction), intra
@@ -285,11 +292,11 @@ static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd
 		int ib = (nmb + INTER_CHUNK - 1) / INTER_CHUNK;
 		if (ib > cap) ib = cap;
 #if INTER_WARPS == 4
-		if (minb >= 8) e264_inter4_kernel<8><<<ib, INTER_WARPS * 32, sizeof(InterSmem), c->stream>>>(J);
-		else if (minb >= 6) e264_inter4_kernel<6><<<ib, INTER_WARPS * 32, sizeof(InterSmem), c->stream>>>(J);
+		if (minb >= 8) e264_inter4_kernel<8, LUMA><<<ib, INTER_WARPS * 32, sizeof(InterSmem), c->stream>>>(J);
+		else if (minb >= 6) e264_inter4_kernel<6, LUMA><<<ib, INTER_WARPS * 32, sizeof(InterSmem), c->stream>>>(J);
 		else
 #endif
-		e264_inter4_kernel<INTER_MINB0><<<ib, INTER_WARPS * 32, sizeof(InterSmem), c->stream>>>(J);
+		e264_inter4_kernel<INTER_MINB0, LUMA><<<ib, INTER_WARPS * 32, sizeof(InterSmem), c->stream>>>(J);
 		c->launches++;
 		if (J.err_pic) {   /* the error map of the inter macroblocks, before the intra kernels read it */
 			int mb_blocks = (nmb + MAP_WARPS - 1) / MAP_WARPS;
@@ -300,28 +307,37 @@ static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd
 	if (pd->n_intra > 0 && (mask & 2)) {
 		if (J.rows_mode) {   /* intra pictures: bands of rows, hand-over through shared memory */
 			const int nb = (J.h_mbs + IR_ROWS - 1) / IR_ROWS;
-			if (J.err_pic) e264_intra_rows_kernel<true><<<nb, IR_ROWS * 64, sizeof(IntraRowsSmem), c->stream>>>(J);
-			else e264_intra_rows_kernel<false><<<nb, IR_ROWS * 64, sizeof(IntraRowsSmem), c->stream>>>(J);
+			if (J.err_pic) e264_intra_rows_kernel<true, LUMA><<<nb, IR_ROWS * 64, sizeof(IntraRowsSmem), c->stream>>>(J);
+			else e264_intra_rows_kernel<false, LUMA><<<nb, IR_ROWS * 64, sizeof(IntraRowsSmem), c->stream>>>(J);
 		} else {
 			/* a warp takes several list entries (E264B_INTRA_DIV, default 2): see INTRA_WARPS */
 			static int idiv = -1;
 			if (idiv < 0) { const char *e = getenv("E264B_INTRA_DIV"); idiv = e && atoi(e) > 0 ? atoi(e) : 2; }
 			int ib = (pd->n_intra + INTRA_WARPS * idiv - 1) / (INTRA_WARPS * idiv);
 			if (ib > cap) ib = cap;
-			if (J.err_pic) e264_intra_kernel<true><<<ib, INTRA_WARPS * 32, sizeof(IntraTkSmem), c->stream>>>(J);
-			else e264_intra_kernel<false><<<ib, INTRA_WARPS * 32, sizeof(IntraTkSmem), c->stream>>>(J);
+			if (J.err_pic) e264_intra_kernel<true, LUMA><<<ib, INTRA_WARPS * 32, sizeof(IntraTkSmem), c->stream>>>(J);
+			else e264_intra_kernel<false, LUMA><<<ib, INTRA_WARPS * 32, sizeof(IntraTkSmem), c->stream>>>(J);
 		}
 		c->launches++;
 	}
-	if (with_deblock && (mask & 4)) {      /* one block per band of 16 rows and kind of plane */
-		const int bands = (J.h_mbs + 2 * DBK_PAIRS - 1) / (2 * DBK_PAIRS);
-		if (dm >= 5) e264_deblock_kernel<5><<<2 * bands, DBK_PAIRS * 32, dbk_smem, c->stream>>>(J);
-		else if (dm == 4) e264_deblock_kernel<4><<<2 * bands, DBK_PAIRS * 32, dbk_smem, c->stream>>>(J);
-		else e264_deblock_kernel<2><<<2 * bands, DBK_PAIRS * 32, dbk_smem, c->stream>>>(J);
+	if (with_deblock && (mask & 4)) {      /* one block per band of 16 rows and kind of plane (luma only: per band) */
+		const int bands = (J.h_mbs + 2 * DBK_PAIRS - 1) / (2 * DBK_PAIRS), nb = LUMA ? bands : 2 * bands;
+		if (dm >= 5) e264_deblock_kernel<5, LUMA><<<nb, DBK_PAIRS * 32, dbk_smem, c->stream>>>(J);
+		else if (dm == 4) e264_deblock_kernel<4, LUMA><<<nb, DBK_PAIRS * 32, dbk_smem, c->stream>>>(J);
+		else e264_deblock_kernel<2, LUMA><<<nb, DBK_PAIRS * 32, dbk_smem, c->stream>>>(J);
 		c->launches++;
 	}
 	CK(cudaGetLastError());
 	return 0;
+}
+
+static int launch_picture(E264bDevice *c, const PicJob &J, const E264PicDesc *pd, int with_deblock) {
+	if (!pd->luma_only) return launch_kernels<false>(c, J, pd, with_deblock);
+	/* luma only: the kernels leave the chroma plane alone, it holds 128 (include/edge264_luma.h).  Issued here so that a
+	 * kernel-only replay repeats it with the kernels */
+	uint8_t *f = c->d_frames + (size_t)pd->dst_slot * pd->frame_bytes;
+	CK(cudaMemsetAsync(f + pd->plane_y, 128, (size_t)(pd->frame_bytes - pd->plane_y), c->stream));
+	return launch_kernels<true>(c, J, pd, with_deblock);
 }
 
 /* the packed output of the picture in frame slot pd->dst_slot into d_packed: one launch over all planes */

@@ -269,7 +269,9 @@ __device__ __forceinline__ void clear_residual(WarpSmem *ws, int lane) {
 	if (lane < 16) ((uint4 *)ws->res)[32 + lane] = make_uint4(0, 0, 0, 0);
 }
 
-/* cf: this macroblock's coefficient run, staged in shared memory by the caller (cp.async.bulk) */
+/* cf: this macroblock's coefficient run, staged in shared memory by the caller (cp.async.bulk).  LUMA (luma-only
+ * pictures): the luma residual only; chroma coded bits and levels a record may still carry are skipped. */
+template <bool LUMA>
 __device__ __noinline__ void residual_stage(WarpSmem *ws, const E264MbRec *r, const E264SliceRec *sr, const int16_t *cf, int lane) {
 	clear_residual(ws, lane);
 	const unsigned coded = r->coded;
@@ -296,8 +298,8 @@ __device__ __noinline__ void residual_stage(WarpSmem *ws, const E264MbRec *r, co
 	const int n_luma = (r->flags & MBF_T8x8) ? 64 * __popc(coded & 0x1111) : 16 * __popc(coded & 0xffff);
 	const int16_t *cf_luma = cf;
 	cf += n_luma;
-	const bool any_cdc = (coded & (CODED_CB_DC | CODED_CR_DC)) != 0;
-	if (lane >= 16 && lane < 24) {
+	const bool any_cdc = !LUMA && (coded & (CODED_CB_DC | CODED_CR_DC)) != 0;
+	if (!LUMA && lane >= 16 && lane < 24) {
 		int pl = (lane - 16) >> 2, i = lane & 3, v = 0;
 		if (any_cdc) {
 			int a = cf[4 * pl], b = cf[4 * pl + 1], c = cf[4 * pl + 2], d = cf[4 * pl + 3];
@@ -359,7 +361,7 @@ __device__ __noinline__ void residual_stage(WarpSmem *ws, const E264MbRec *r, co
 				src = cf_luma + __popc(coded & ((1u << b) - 1)) * 16; scal = sr->scaling4x4[inter * 3]; dcov = i16; dc = ws->dc[by * 4 + bx];
 				dst = ws->res + by * 4 * 16 + bx * 4;
 			}
-		} else if (lane < 24) {
+		} else if (!LUMA && lane < 24) {
 			const int j = lane - 16, pl = j >> 2, i = j & 3;
 			on = (coded >> (16 + j)) & 1; act = on || any_cdc; dcov = true;
 			src = cf + __popc((coded >> 16) & ((1u << j) - 1) & 0xff) * 16; scal = sr->scaling4x4[1 + pl + inter * 3]; qp = r->qp[1 + pl]; dc = ws->dc[16 + pl * 4 + i];
@@ -571,22 +573,25 @@ __device__ __forceinline__ void mb_planes(const PicJob &J, int mbx, int mby, uin
 }
 /* the row above the macroblock from the picture into tile row -1 (luma x = -1..23, chroma x = -1..7; x = -1 only with
  * `left`, luma x >= 16 only with `right`): Ya, Ca point at sample (0, -1) of luma and of Cb, Cr follows cpl bytes further */
+template <bool LUMA>
 __device__ __forceinline__ void load_row_above(WarpSmem *ws, const uint8_t *Ya, const uint8_t *Ca, int cpl, bool left, bool right, int lane) {
 	const int x = lane - 1;
 	if (x < 24 && (x >= 0 || left) && (x < 16 || right)) YT(x, -1) = __ldcg(Ya + x);
-	if (lane < 18) { const int pl = lane / 9, cx = lane % 9 - 1; if (cx >= 0 || left) CT(pl, cx, -1) = __ldcg(Ca + pl * cpl + cx); }
+	if (!LUMA && lane < 18) { const int pl = lane / 9, cx = lane % 9 - 1; if (cx >= 0 || left) CT(pl, cx, -1) = __ldcg(Ca + pl * cpl + cx); }
 }
-/* the raw samples of an I_PCM macroblock (its 384-byte "coefficient run") into the tile */
+/* the raw samples of an I_PCM macroblock (its 384-byte "coefficient run") into the tile (LUMA: the 256 luma ones) */
+template <bool LUMA>
 __device__ __forceinline__ void load_pcm(WarpSmem *ws, const PicJob &J, const E264MbRec *r, int lane) {
 	const uint8_t *s = (const uint8_t *)(J.coefs + r->coef_off);
 	if (lane < 16) *(uint4 *)&YT(0, lane) = __ldg((const uint4 *)s + lane);
-	else { const int j = lane - 16; *(uint2 *)&CT(j >> 3, 0, j & 7) = __ldg((const uint2 *)(s + 256) + j); }
+	else if (!LUMA) { const int j = lane - 16; *(uint2 *)&CT(j >> 3, 0, j & 7) = __ldg((const uint2 *)(s + 256) + j); }
 	__syncwarp();
 }
+template <bool LUMA>
 __device__ __forceinline__ void store_mb(WarpSmem *ws, const PicJob &J, uint8_t *Y, uint8_t *C, int lane) {
 	const int cpl = J.stride_c >> 1;
 	if (lane < 16) *(uint4 *)(Y + (size_t)lane * J.stride_y) = *(const uint4 *)&YT(0, lane);
-	else { int j = lane - 16, pl = j >> 3, row = j & 7; *(uint2 *)(C + pl * cpl + (size_t)row * J.stride_c) = *(const uint2 *)&CT(pl, 0, row); }
+	else if (!LUMA) { int j = lane - 16, pl = j >> 3, row = j & 7; *(uint2 *)(C + pl * cpl + (size_t)row * J.stride_c) = *(const uint2 *)&CT(pl, 0, row); }
 }
 
 #define RES_COEF_MAX 416   /* 16 + 256 + 8 + 128 levels, rounded up */

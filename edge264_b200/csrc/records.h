@@ -124,9 +124,15 @@ typedef struct E264PicDesc {
 	int32_t any_deblock;          /* at least one macroblock has MBF_DEBLOCK */
 	int32_t n_intra;              /* number of intra macroblocks = entries of the staging's intra_list */
 	int32_t staging;              /* handle of the staging area the picture was written into (E264Staging.handle) */
-	int32_t err_pic;              /* error map wanted: some record has err != 0 or a slot in taint is referenced; with 0 the
+	uint8_t err_pic;              /* error map wanted: some record has err != 0 or a slot in taint is referenced; with 0 the
 	                               * kernels touch no map and the slot's map counts as all zeros afterwards */
-	uint32_t taint;               /* bit s: frame slot s holds a picture whose map may be nonzero (fill_slot, err_pic) */
+	uint8_t luma_only;            /* reconstruct and deblock the Y plane only, then set the slot's chroma plane to 128
+	                               * (include/edge264_luma.h); the chroma levels and coded bits of the records are ignored.
+	                               * The parser's records of such pictures reconstruct chroma 128 anyway (decoder.c
+	                               * edge264_enable_luma_only), so a backend that ignores this field gives the same frame */
+	uint8_t reserved[2];          /* (err_pic and luma_only share the word err_pic had: the struct stays 56 bytes, the size
+	                               * the picture dumps of the deblocking tests are read with) */
+	uint32_t taint;              /* bit s: frame slot s holds a picture whose map may be nonzero (fill_slot, err_pic) */
 } E264PicDesc;
 
 /* The motion export of one picture (include/edge264_motion.h): one buffer of E264_MOTION_BYTES bytes per macroblock, the

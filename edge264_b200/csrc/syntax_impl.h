@@ -624,6 +624,7 @@ static void sx_residual(SliceCtx *s, int is_i16, int cbp) {
 		}
 	}
 	if (cbp >> 4) {
+		const uint32_t chroma_off = s->n_coefs;
 		int16_t *dc = sx_pool_take(s, 8, 272);
 		int any = 0;
 		for (int pl = 0; pl < 2; pl++) {
@@ -646,6 +647,9 @@ static void sx_residual(SliceCtx *s, int is_i16, int cbp) {
 				if (n) coded |= 1u << (16 + pl * 4 + i); else s->n_coefs -= 16;
 			}
 		}
+		/* luma only: every chroma element is parsed above (the entropy state and the neighbours' cbf / tc need it), then
+		 * its levels leave the pool again (they are the run's tail) and the record keeps no chroma bit */
+		if (s->luma_only) { s->n_coefs = chroma_off; coded &= 0xffffu | CODED_Y_DC; }
 	}
 	r->coded = coded;
 }

@@ -12,6 +12,9 @@
 #include <time.h>
 #include "edge264.h"
 
+/* include/edge264_luma.h; weak: the reference's library has no such entry point */
+int edge264_enable_luma_only(Edge264Decoder *dec) __attribute__((weak));
+
 typedef struct Job {
 	const uint8_t *buf; size_t size;
 	long frames; uint64_t sum; int last_ret;
@@ -43,6 +46,9 @@ static void decode_stream(Job *j) {
 	Edge264Decoder *dec = edge264_alloc(nt ? atoi(nt) : 0, NULL, NULL, 0, NULL, NULL, NULL);
 	Edge264Frame f; int res, drained = 0; long frames = 0; uint64_t sum = 0;
 	if (!dec) { j->last_ret = -1; return; }
+	/* E264_BENCH_LUMA_ONLY=1: every decoder decodes the Y plane only (tools/luma_only_cost.py) */
+	const char *lo = getenv("E264_BENCH_LUMA_ONLY");
+	if (lo && atoi(lo) && (!edge264_enable_luma_only || edge264_enable_luma_only(dec))) { edge264_free(&dec); j->last_ret = -1; return; }
 	for (;;) {
 		const uint8_t *sc = nal < end ? edge264_find_start_code(nal, end, 0) : end;
 		long before = frames;
