@@ -40,6 +40,12 @@ class Edge264Packed(ctypes.Structure):
                 ("on_device", ctypes.c_int32)]
 
 
+class Edge264PicStats(ctypes.Structure):
+    """Layout of include/edge264_picstats.h: one frame's statistics (pointers into the decoder's buffer of that frame)."""
+    _fields_ = [("hist", ctypes.POINTER(ctypes.c_uint32)), ("sum", ctypes.POINTER(ctypes.c_uint32)), ("sum_sq", ctypes.POINTER(ctypes.c_uint32)),
+                ("width_mbs", ctypes.c_int32), ("height_mbs", ctypes.c_int32), ("on_device", ctypes.c_int32)]
+
+
 SKIP_NONE, SKIP_NONREF, SKIP_NONKEY = 0, 1, 2   # include/edge264_skip.h
 
 
@@ -79,6 +85,9 @@ def bind(path):
         lib.edge264_set_skip.argtypes = [ctypes.c_void_p, ctypes.c_int]
     if hasattr(lib, "edge264_enable_luma_only"):   # the extension of include/edge264_luma.h
         lib.edge264_enable_luma_only.argtypes = [ctypes.c_void_p]
+    if hasattr(lib, "edge264_get_picstats"):   # the extension of include/edge264_picstats.h
+        lib.edge264_enable_picstats.argtypes = [ctypes.c_void_p]
+        lib.edge264_get_picstats.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264PicStats)]
     _loaded[path] = lib
     return lib
 
@@ -157,14 +166,37 @@ def frame_packed(lib, dec, f):
     return out
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False):
+def frame_picstats(lib, dec, f):
+    """The statistics of frame f (just returned by edge264_get_frame) as a dict of numpy uint32 arrays (copies): hist
+    [3][256], sum [3][H][W], sum_sq [3][H][W], and on_device.  Device memory is copied through torch."""
+    import numpy as np
+    s = Edge264PicStats()
+    r = lib.edge264_get_picstats(dec, ctypes.byref(f), ctypes.byref(s))
+    if r:
+        raise RuntimeError("edge264_get_picstats: %s" % errno.errorcode.get(r, r))
+    W, H = s.width_mbs, s.height_mbs
+    out = {"on_device": s.on_device}
+    for k, shape in (("hist", (3, 256)), ("sum", (3, H, W)), ("sum_sq", (3, H, W))):
+        ptr = ctypes.cast(getattr(s, k), ctypes.c_void_p).value
+        n = 4 * int(np.prod(shape))
+        if s.on_device:
+            import torch
+            raw = torch.as_tensor(_DeviceBytes(ptr, n), device="cuda").cpu().numpy()
+        else:
+            raw = np.frombuffer(ctypes.string_at(ptr, n), np.uint8)
+        out[k] = raw.view(np.uint32).reshape(shape)
+    return out
+
+
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False, picstats=False):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
     carries the frame's motion export (frame_motion); with packed=(format, log2_scale) it ends with the frame's packed
     output (frame_packed); resized=(format, width, height) does the same with the resized output (edge264_enable_resized,
     log2_scale -1); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip); luma_only=True decodes
-    the Y plane only, chroma comes out as 128 (edge264_enable_luma_only)."""
+    the Y plane only, chroma comes out as 128 (edge264_enable_luma_only); picstats=True appends the frame's statistics
+    (frame_picstats) as the last element of each frame tuple."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -203,6 +235,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             d = ctypes.c_void_p(dec)
             lib.edge264_free(ctypes.byref(d))
             raise RuntimeError("edge264_enable_luma_only: %s" % errno.errorcode.get(r, r))
+    if picstats:
+        r = lib.edge264_enable_picstats(dec) if hasattr(lib, "edge264_enable_picstats") else errno.ENOTSUP
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_enable_picstats: %s" % errno.errorcode.get(r, r))
     nal = base + 3 + (1 if data[2] == 0 else 0)
     frames, codes, f = [], [], Edge264Frame()
     drained = False
@@ -214,7 +252,8 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             drained = True
         while lib.edge264_get_frame(dec, ctypes.byref(f), 0) == 0:
             frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ())
-                          + ((frame_motion(lib, dec, f),) if motion else ()) + ((frame_packed(lib, dec, f),) if packed is not None or resized is not None else ()))
+                          + ((frame_motion(lib, dec, f),) if motion else ()) + ((frame_packed(lib, dec, f),) if packed is not None or resized is not None else ())
+                          + ((frame_picstats(lib, dec, f),) if picstats else ()))
         if res == errno.ENOBUFS:
             if len(frames) == before:
                 break

@@ -186,6 +186,9 @@ typedef struct HostBuf {
 	void *packed_mbs;     /* the mbs allocation alloc_cb returned with it */
 	int packed_dev;       /* packed is device memory */
 	E264PackedDesc pk;    /* what the picture in the buffer was packed as (cropping rectangle and resized size of its sequence) */
+	uint8_t *picstats;    /* the picture's statistics (records.h E264_PICSTATS_*), memory of the samples' kind; NULL without them */
+	void *picstats_mbs;   /* the mbs allocation alloc_cb returned with it */
+	int picstats_dev;     /* picstats is device memory */
 	int state;            /* 0 free, 1 attached to a decoded picture, 2 in the output queue, 3 handed out */
 	int borrowed;
 	int32_t frame_id;
@@ -234,10 +237,11 @@ struct Edge264Decoder {
 	int pending_release;               /* host buffer handed out without borrow, released at next decode_NAL */
 	int sync_output;                   /* E264_SYNC_OUTPUT=1: get_frame always waits for the device (the behaviour before round 2's last step; A/B switch) */
 	int motion;                        /* edge264_enable_motion: every output picture carries its motion export */
-	int slices_seen;                   /* a slice NAL unit has been decoded (edge264_enable_motion / _packed / _resized are refused from then on) */
+	int slices_seen;                   /* a slice NAL unit has been decoded (edge264_enable_motion / _packed / _resized / _picstats are refused from then on) */
 	int packed, packed_format, packed_scale;   /* edge264_enable_packed: every output picture carries its packed output */
 	int packed_width, packed_height;   /* edge264_enable_resized (packed_scale -1): the requested size, one of them possibly 0 */
 	int luma_only;                     /* edge264_enable_luma_only: every picture is reconstructed with luma only */
+	int picstats;                      /* edge264_enable_picstats: every output picture carries its statistics */
 	int block_output;                  /* the last decode_NAL asked the application to fetch frames (ENOBUFS, end of stream): get_frame waits for the device */
 	/* scratch: RBSP of the last non-slice NAL unit */
 	uint8_t *rbsp; size_t rbsp_cap;

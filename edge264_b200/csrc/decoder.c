@@ -17,6 +17,7 @@
 #include "h264_tables.h"
 #include "../../include/edge264_motion.h"
 #include "../../include/edge264_packed.h"
+#include "../../include/edge264_picstats.h"
 #include "../../include/edge264_skip.h"
 #include "../../include/edge264_luma.h"
 
@@ -250,6 +251,10 @@ static void hostbuf_free(Edge264Decoder *d, HostBuf *hb) {
 		if (d->alloc_cb) d->free_cb(hb->packed, hb->packed_mbs, d->alloc_arg);
 		else d->be->host_free(d->be_ctx, hb->packed);
 	}
+	if (hb->picstats) {
+		if (d->alloc_cb) d->free_cb(hb->picstats, hb->picstats_mbs, d->alloc_arg);
+		else d->be->host_free(d->be_ctx, hb->picstats);
+	}
 	memset(hb, 0, sizeof(*hb));
 }
 /* the nearest even size to s_a * t_b / s_b, within 2..16384: the resized side that keeps the aspect ratio */
@@ -305,12 +310,13 @@ static int hostbuf_acquire(Edge264Decoder *d) {
 			pthread_mutex_unlock(&d->be_lock);
 			if (!hb->map) { hostbuf_free(d, hb); return -1; }
 		}
-		/* the motion export and the packed output live where the samples live */
+		/* the motion export, the packed output and the statistics live where the samples live */
 		if (d->motion && !(hb->motion = side_alloc(d, (size_t)d->w_mbs * d->h_mbs * E264_MOTION_BYTES, &hb->motion_mbs))) { hostbuf_free(d, hb); return -1; }
 		if (d->packed) {
 			const E264PackedDesc k = packed_desc(d);
 			if (!(hb->packed = side_alloc(d, (size_t)e264_packed_layout(&k).bytes, &hb->packed_mbs))) { hostbuf_free(d, hb); return -1; }
 		}
+		if (d->picstats && !(hb->picstats = side_alloc(d, E264_PICSTATS_BYTES((size_t)d->w_mbs * d->h_mbs), &hb->picstats_mbs))) { hostbuf_free(d, hb); return -1; }
 		return i;
 	}
 	return -1;
@@ -431,9 +437,11 @@ static int build_submit(Edge264Decoder *d, PicBuild *pb, E264PicDesc *pd, uint64
 	int r;
 	{
 		PROF_BEGIN;
-		if (d->packed) {   /* the picture is packed when it is reconstructed, like its samples are copied then */
-			hb->pk = packed_desc(d);
-			const E264Outputs o = {hb->map, hb->motion, pb->slot_ids, E264_MAX_SLOTS, &hb->motion_dev, hb->packed, hb->pk, &hb->packed_dev};
+		if (d->packed || d->picstats) {   /* the picture is packed and measured when it is reconstructed, like its samples are copied then */
+			const E264PackedDesc k = packed_desc(d);   /* the statistics' histograms take its cropping rectangle */
+			if (d->packed) hb->pk = k;
+			const E264Outputs o = {hb->map, hb->motion, pb->slot_ids, E264_MAX_SLOTS, &hb->motion_dev, hb->packed, hb->pk, &hb->packed_dev,
+			                       hb->picstats, k.left, k.top, k.width, k.height, &hb->picstats_dev};
 			r = d->be->submit_outputs(d->be_ctx, pd, hb->p, &o, ticket);
 		} else if (d->motion) r = d->be->submit_motion(d->be_ctx, pd, hb->p, hb->map, hb->motion, pb->slot_ids, &hb->motion_dev, ticket);
 		else r = d->be->submit_maps ? d->be->submit_maps(d->be_ctx, pd, hb->p, hb->map, ticket) : d->be->submit(d->be_ctx, pd, hb->p, ticket);
@@ -1406,6 +1414,32 @@ int edge264_get_packed(Edge264Decoder *d, const Edge264Frame *frame, Edge264Pack
 	out->width = l.width; out->height = l.height; out->width_C = l.width_C; out->height_C = l.height_C;
 	out->format = hb->pk.format; out->log2_scale = hb->pk.log2_scale;
 	out->on_device = hb->packed_dev;
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* picture statistics (include/edge264_picstats.h)                                              */
+/* ------------------------------------------------------------------------------------------ */
+int edge264_enable_picstats(Edge264Decoder *d) {
+	if (!d) return EINVAL;
+	if (!d->be->submit_outputs) return ENOTSUP;
+	if (d->slices_seen) return EBUSY;   /* host buffers are created with the first picture: they would lack the statistics */
+	d->picstats = 1;
+	return 0;
+}
+
+int edge264_get_picstats(Edge264Decoder *d, const Edge264Frame *frame, Edge264PicStats *out) {
+	if (!d || !frame || !out) return EINVAL;
+	if (!d->picstats) return ENOENT;
+	const int i = (int)(uintptr_t)frame->return_arg - 1;
+	if (i < 0 || i >= E264_MAX_HOSTBUFS || d->hb[i].state != 3 || !d->hb[i].picstats) return EINVAL;
+	const size_t nmb = (size_t)d->w_mbs * d->h_mbs;
+	const uint8_t *s = d->hb[i].picstats;
+	out->hist = (const uint32_t *)(s + E264_PICSTATS_HIST);
+	out->sum = (const uint32_t *)(s + E264_PICSTATS_SUM);
+	out->sum_sq = (const uint32_t *)(s + E264_PICSTATS_SUM_SQ(nmb));
+	out->width_mbs = d->w_mbs; out->height_mbs = d->h_mbs;
+	out->on_device = d->hb[i].picstats_dev;
 	return 0;
 }
 

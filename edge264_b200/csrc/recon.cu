@@ -23,6 +23,7 @@
 #include "motion_kernels.cuh"
 #include "pack_kernels.cuh"
 #include "resize_kernels.cuh"
+#include "picstats_kernels.cuh"
 extern "C" {
 #include "dec.h"
 }
@@ -47,6 +48,7 @@ struct E264bDevice {
 	uint8_t *d_maps;             /* [n_slots][nmb] error maps of the frame slots (written only for pictures with err_pic) */
 	uint8_t *d_motion;           /* [nmb * E264_MOTION_BYTES] motion export of the picture last submitted with one (allocated at the first) */
 	uint8_t *d_packed; size_t packed_cap;   /* packed output of the picture last submitted with one (allocated at the first, grown when a layout needs more) */
+	uint8_t *d_picstats;         /* [E264_PICSTATS_BYTES(nmb)] statistics of the picture last submitted with them (allocated at the first) */
 	E264MbRec *h_recs[E264_MAX_SLOTS]; cudaEvent_t rec_up[E264_MAX_SLOTS]; bool rec_busy[E264_MAX_SLOTS];
 	Staging st[NSTAGE]; int stage, n_stage;
 	unsigned *d_sync;            /* synchronisation words, layout SYNC_* in recon_kernels.cuh */
@@ -80,6 +82,8 @@ static void free_geometry(E264bDevice *c) {
 	c->d_motion = NULL;
 	if (c->d_packed) cudaFree(c->d_packed);
 	c->d_packed = NULL; c->packed_cap = 0;
+	if (c->d_picstats) cudaFree(c->d_picstats);
+	c->d_picstats = NULL;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { if (c->h_recs[i]) cudaFreeHost(c->h_recs[i]); c->h_recs[i] = NULL; c->rec_busy[i] = false; }
 	for (int i = 0; i < NSTAGE; i++) {
 		Staging *s = &c->st[i];
@@ -420,7 +424,7 @@ extern "C" int e264b_submit_motion(E264bDevice *c, const E264PicDesc *pd, uint8_
 	return e264b_submit_outputs(c, pd, host_out, &o, ticket);
 }
 extern "C" int e264b_submit_outputs(E264bDevice *c, const E264PicDesc *pd, uint8_t *host_out, const E264Outputs *o, uint64_t *ticket) {
-	uint8_t *const host_map = o->map, *const motion = o->motion, *const packed = o->packed;
+	uint8_t *const host_map = o->map, *const motion = o->motion, *const packed = o->packed, *const picstats = o->picstats;
 	const int32_t *const slot_ids = o->slot_ids; const int n_ids = o->n_ids;
 	E264PackedLayout pl; memset(&pl, 0, sizeof(pl));
 	if (packed) {
@@ -433,6 +437,8 @@ extern "C" int e264b_submit_outputs(E264bDevice *c, const E264PicDesc *pd, uint8
 		            : k->log2_scale < 0 || k->log2_scale > 3) return -1;
 		pl = e264_packed_layout(k);
 	}
+	if (picstats && (((o->ps_left | o->ps_top | o->ps_width | o->ps_height) & 1) || o->ps_left < 0 || o->ps_top < 0 || o->ps_width < 2 || o->ps_height < 2 ||
+	                 o->ps_left + o->ps_width > pd->width_mbs * 16 || o->ps_top + o->ps_height > pd->height_mbs * 16)) return -1;
 	CK(cudaSetDevice(c->dev));
 	if (motion && (n_ids < 0 || n_ids > MOTION_MAX_SLOTS)) return -1;
 	if (pd->staging < 0 || pd->staging >= c->n_stage) return -1;
@@ -482,6 +488,20 @@ extern "C" int e264b_submit_outputs(E264bDevice *c, const E264PicDesc *pd, uint8
 		if ((o->pk.target_width ? resize_picture(c, pd, &o->pk, pl) : pack_picture(c, pd, &o->pk, pl))) return -1;
 		CK(cudaMemcpyAsync(packed, c->d_packed, pl.bytes, cudaMemcpyDefault, c->stream)); c->d2h_bytes += pl.bytes;
 		if (o->packed_on_device) *o->packed_on_device = is_device_memory(packed);
+	}
+	if (picstats) {   /* the picture statistics, from the finished frame slot, through a scratch like the motion export */
+		const size_t bytes = E264_PICSTATS_BYTES(c->nmb);
+		if (!c->d_picstats) CK(cudaMalloc(&c->d_picstats, bytes));
+		CK(cudaMemsetAsync(c->d_picstats + E264_PICSTATS_HIST, 0, 3 * 256 * sizeof(uint32_t), c->stream));
+		const uint8_t *slot = c->d_frames + (size_t)pd->dst_slot * pd->frame_bytes;
+		const PicStatsArgs A = {slot, slot + pd->plane_y, pd->stride_y, pd->stride_c, pd->width_mbs, pd->height_mbs,
+		                        o->ps_left, o->ps_top, o->ps_left + o->ps_width, o->ps_top + o->ps_height, (uint32_t *)c->d_picstats};
+		const int blocks = (int)((c->nmb + PS_WARPS - 1) / PS_WARPS);
+		e264_picstats_kernel<<<blocks < 2 * c->sm_count ? blocks : 2 * c->sm_count, PS_THREADS, 0, c->stream>>>(A);
+		c->launches++;
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(picstats, c->d_picstats, bytes, cudaMemcpyDefault, c->stream)); c->d2h_bytes += bytes;
+		if (o->picstats_on_device) *o->picstats_on_device = is_device_memory(picstats);
 	}
 	if (c->keep) {
 		KeptPic k; k.pd = *pd;

@@ -8,6 +8,7 @@
  *   motion_kernels.cuh   e264_motion_kernel      the motion export (decoders that asked for it): records -> raster arrays
  *   pack_kernels.cuh     e264_pack_kernel        the packed output (decoders that asked for it): frame slot -> cropped I420 / NV12, box-downscaled
  *   resize_kernels.cuh   e264_resize_kernel      the resized output (decoders that asked for it): frame slot -> cropped I420 / NV12, any size, area-averaged
+ *   picstats_kernels.cuh e264_picstats_kernel    the picture statistics (decoders that asked for them): frame slot -> histograms, per-macroblock sums
  * Up to three launches per picture.  Arithmetic is restated from ITU-T H.264 with the reference's observable integer
  * widths; results are bit-exact with the reference decoder (tests/test_gpu_parity.py). */
 #pragma once

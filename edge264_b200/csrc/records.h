@@ -47,6 +47,7 @@
  */
 #ifndef E264B_RECORDS_H
 #define E264B_RECORDS_H
+#include <stddef.h>
 #include <stdint.h>
 
 /* widest picture the parser accepts, in macroblocks: the device's row-progress words count a row's macroblocks below
@@ -143,6 +144,14 @@ typedef struct E264PicDesc {
  *   mb_qp         E264_MOTION_QP * nmb    uint8 [height_mbs][width_mbs] */
 enum { E264_MOTION_MV = 0, E264_MOTION_REF = 128, E264_MOTION_TYPE = 160, E264_MOTION_QP = 161, E264_MOTION_BYTES = 162 };
 
+/* The picture statistics of one picture (include/edge264_picstats.h): one buffer of E264_PICSTATS_BYTES(nmb) bytes,
+ *   hist    at E264_PICSTATS_HIST                uint32 [3][256]
+ *   sum     at E264_PICSTATS_SUM                 uint32 [3][height_mbs][width_mbs]
+ *   sum_sq  at E264_PICSTATS_SUM + 12 * nmb      uint32 [3][height_mbs][width_mbs] */
+enum { E264_PICSTATS_HIST = 0, E264_PICSTATS_SUM = 3072, E264_PICSTATS_MB_BYTES = 24 };
+#define E264_PICSTATS_SUM_SQ(nmb) (E264_PICSTATS_SUM + 12 * (size_t)(nmb))
+#define E264_PICSTATS_BYTES(nmb) (E264_PICSTATS_SUM + E264_PICSTATS_MB_BYTES * (size_t)(nmb))
+
 /* The packed output of one picture (include/edge264_packed.h): the cropped picture as I420 or NV12, box-downscaled by
  * 1 << log2_scale, or resized to target_width x target_height, in one buffer.  E264PackedDesc says what to pack,
  * e264_packed_layout where every plane goes: sizes are ceil(cropped size / scale), or the target (chroma: half of it), a
@@ -180,12 +189,14 @@ static inline E264PackedLayout e264_packed_layout(const E264PackedDesc *p) {
 
 /* What a submit may produce besides the samples; a NULL pointer leaves that output out (no launch, no copy, no
  * allocation for it).  map: the error map, copied when pd->err_pic.  motion: the motion export, slot_ids[s] the FrameId
- * of frame slot s for s < n_ids, -1 elsewhere.  packed: the packed output described by pk.  The *_on_device words (may be
- * NULL) receive whether that destination is device memory. */
+ * of frame slot s for s < n_ids, -1 elsewhere.  packed: the packed output described by pk.  picstats: the picture
+ * statistics, the histograms over the cropping rectangle ps_left, ps_top, ps_width x ps_height (luma samples inside the
+ * coded picture, all even).  The *_on_device words (may be NULL) receive whether that destination is device memory. */
 typedef struct E264Outputs {
 	uint8_t *map;
 	uint8_t *motion; const int32_t *slot_ids; int32_t n_ids; int *motion_on_device;
 	uint8_t *packed; E264PackedDesc pk; int *packed_on_device;
+	uint8_t *picstats; int32_t ps_left, ps_top, ps_width, ps_height; int *picstats_on_device;
 } E264Outputs;
 
 /* Host-visible staging of one picture, handed out by the backend (pinned memory for the CUDA backend): the parser

@@ -44,10 +44,13 @@ int   e264b_submit_maps(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t
 int   e264b_submit_motion(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, uint8_t *host_map, uint8_t *motion,
                           const int32_t *slot_ids, int n_ids, int *on_device, uint64_t *ticket);
 /* The one submit the three above are thin callers of: `out` (struct E264Outputs of edge264_b200/csrc/records.h) names the
- * optional outputs, each left out when its pointer is NULL: the error map, the motion export, and the packed output
+ * optional outputs, each left out when its pointer is NULL: the error map, the motion export, the packed output
  * (include/edge264_packed.h: the cropped picture as I420 or NV12, optionally box-downscaled, written by e264_pack_kernel,
  * or resized to out->pk's target size by exact area averaging, written by e264_resize_kernel; with the layout of
- * e264_packed_layout; one launch and one copy of that many bytes per picture). */
+ * e264_packed_layout; one launch and one copy of that many bytes per picture), and the picture statistics
+ * (include/edge264_picstats.h: histograms over out's cropping rectangle, per-macroblock sums and sums of squares, written
+ * by e264_picstats_kernel with the layout E264_PICSTATS_*; one memset, one launch and one copy of
+ * E264_PICSTATS_BYTES(nmb) bytes per picture). */
 int   e264b_submit_outputs(E264bDevice *dev, const struct E264PicDesc *pic, uint8_t *host_out, const struct E264Outputs *out, uint64_t *ticket);
 int   e264b_wait(E264bDevice *dev, uint64_t ticket);
 int   e264b_poll(E264bDevice *dev, uint64_t ticket);          /* 0 complete, EAGAIN still on the device, < 0 device error */
