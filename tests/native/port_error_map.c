@@ -1,7 +1,7 @@
 /* port_error_map.c — TEST INFRASTRUCTURE ONLY.  The error-map rules of E264PicDesc.err_pic / taint and E264MbRec.err in
  * plain C, restated from the feature's specification (not from the kernels): what the device's map of every frame slot
- * must hold after every picture.  Built by tests/test_mb_errors.py into the maps-keeping CPU backend
- * (port_maps_backend.c) and into the record fuzzer's error-map driver (record_fuzz_maps.c). */
+ * must hold after every picture.  Built by tests/checkers.py into the CPU backend with every optional output
+ * (port_outputs_backend.c) and by tests/test_mb_errors.py into the record fuzzer's error-map driver (record_fuzz_maps.c). */
 #include <stddef.h>
 #include <stdint.h>
 #include "../../edge264_b200/csrc/records.h"

@@ -3,19 +3,18 @@ of every output frame is 128.  In 4:2:0 8-bit decoding no luma sample depends on
 own full decode (pinned to the reference elsewhere): a luma-only decode must give the same frames, FrameIds, order and
 return codes, the same Y plane byte for byte, chroma all 128, and the same error maps and motion export.
 
-CPU tests run the product's host sources over the plain-C restatement (oracle/liboracle_dec.so, and the test backends
-with error maps, motion export and packed output); the GPU tests compare the device with the device's full decode and
-with the restatement's luma-only decode."""
+CPU tests run the product's host sources over the plain-C restatement (oracle/liboracle_dec.so, and the test backend
+with every optional output, tests/native/port_outputs_backend.c); the GPU tests compare the device with the device's
+full decode and with the restatement's luma-only decode."""
 import ctypes, errno, os, pickle, random, re, subprocess, sys, threading
 from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 from conftest import ROOT, STREAMS, DPB_STREAMS, make_stream, have
 from test_limits import LIMITS, FULL_LIMITS
-from test_robustness import CASES as DAMAGED_CASES, damage
 from test_gpu_parity import FULL
-from test_motion_export import port_motion_lib
-from test_resized_output import port_resized_lib
+from api_helpers import _damaged
+from checkers import port_outputs_lib
 import edge264_b200 as pkg
 import checkers
 
@@ -70,7 +69,7 @@ def test_port_worker_counts_give_identical_output(workdir, stream):
 
 @pytest.mark.parametrize("stream", STREAMS + DPB_STREAMS + LIMITS, ids=[s[0] for s in STREAMS + DPB_STREAMS + LIMITS])
 def test_port_error_maps_and_motion_export_equal_full_decode(workdir, stream):
-    data, lib = _data(workdir, stream), port_motion_lib()
+    data, lib = _data(workdir, stream), port_outputs_lib()
     same_as_full(pkg.decode_bytes(data, lib, errors=True, motion=True), pkg.decode_bytes(data, lib, errors=True, motion=True, luma_only=True), stream[0])
 
 
@@ -82,17 +81,9 @@ def test_port_with_skipped_pictures_equals_skip_decode(workdir, skip):
         same_as_full(pkg.decode_bytes(data, lib, skip=skip), pkg.decode_bytes(data, lib, skip=skip, luma_only=True), s[0])
 
 
-def _damaged(workdir):
-    """The 75 damaged streams of test_robustness.py, same mutations and seeds."""
-    for name, w, h, args in DAMAGED_CASES:
-        src = _data(workdir, (name, w, h, args))
-        for seed in range(25):
-            yield name, seed, damage(src, random.Random(seed * 7919 + len(src)))
-
-
 def test_port_damaged_streams_equal_full_decode_and_keep_the_record_contract(workdir, monkeypatch):
     """Error maps included; with E264_CHECK_RECORDS=1 every luma-only picture submitted keeps the record contract."""
-    lib = port_motion_lib()
+    lib = port_outputs_lib()
     monkeypatch.setenv("E264_CHECK_RECORDS", "1")
     before, n = lib.e264_test_record_violations(), 0
     for name, seed, data in _damaged(workdir):
@@ -138,7 +129,7 @@ def test_api_contract(workdir):
 
 def test_packed_and_resized_outputs_follow_their_definitions(workdir):
     """CPU restatement of the packed and resized outputs: Y plane equal to the full decode's, chroma planes 128."""
-    lib = port_resized_lib()
+    lib = port_outputs_lib()
     for s in (next(x for x in DPB_STREAMS if x[0] == "crop_rect"), next(x for x in STREAMS if x[0] == "b_explicit")):
         data = _data(workdir, s)
         for kw in ({"packed": (pkg.PACKED_NV12, 0)}, {"packed": (pkg.PACKED_NV12, 2)}, {"packed": (pkg.PACKED_I420, 1)},
@@ -224,7 +215,7 @@ def test_device_error_maps_motion_skip_threads_and_damage(workdir):
             same_as_full(pkg.decode_bytes(data, lib, t, errors=True, motion=True), pkg.decode_bytes(data, lib, t, errors=True, motion=True, luma_only=True), s[0])
         for skip in (pkg.SKIP_NONREF, pkg.SKIP_NONKEY):
             same_as_full(pkg.decode_bytes(data, lib, skip=skip), pkg.decode_bytes(data, lib, skip=skip, luma_only=True), s[0])
-    port = port_motion_lib()
+    port = port_outputs_lib()
     for name, seed, data in _damaged(workdir):
         luma = pkg.decode_bytes(data, lib, errors=True, luma_only=True)
         same_as_full(pkg.decode_bytes(data, lib, errors=True), luma, "%s seed %d" % (name, seed))

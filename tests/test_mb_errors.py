@@ -3,11 +3,11 @@ is 0).  Sources: 100 for concealed macroblocks and for inter macroblocks predict
 reference decoder's ramp for the macroblocks a broken slice delivered; the device carries them forward through motion
 vectors and intra neighbours.  CPU tests run the product's host sources over the plain-C restatement of the
 reconstruction (oracle/port_recon.c) and of the error maps (tests/native/port_error_map.c), bound by
-tests/native/port_maps_backend.c into a library built here; the GPU tests compare the device's maps and samples with it."""
-import ctypes, errno, os, random, subprocess, tempfile
+tests/native/port_outputs_backend.c into a library built here; the GPU tests compare the device's maps and samples with it."""
+import ctypes, errno, os, subprocess
 import pytest
 from conftest import ROOT, STREAMS, DPB_STREAMS, make_stream
-from test_robustness import CASES as DAMAGED_CASES, damage
+from api_helpers import lib_of, new_decoder, free_decoder, loop, _ALLOC, _FREE, _cudart, _damaged
 import edge264_b200 as pkg
 import checkers
 
@@ -47,28 +47,10 @@ def _slice_head(nal):
 
 
 NATIVE = os.path.join(ROOT, "tests", "native")
-CSRC = os.path.join(ROOT, "edge264_b200", "csrc")
-_built = {}
-
-
-def port_maps_lib():
-    """The whole edge264 API on the CPU with error maps: the product's host sources over port_maps_backend.c."""
-    if "lib" not in _built:
-        path = os.path.join(tempfile.mkdtemp(prefix="e264maps"), "libport_maps.so")
-        src = [os.path.join(NATIVE, "port_maps_backend.c"), os.path.join(NATIVE, "port_error_map.c"), os.path.join(ROOT, "oracle", "port_recon.c"),
-               os.path.join(ROOT, "oracle", "record_check.c"), os.path.join(CSRC, "decoder.c"), os.path.join(CSRC, "slice_dec.c")]
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-w", "-o", path] + src + ["-pthread"], check=True)
-        lib = pkg.bind(path)
-        lib.e264_test_record_violations.restype = ctypes.c_int
-        lib.e264_test_last_violation.restype = ctypes.c_char_p
-        _built["lib"] = lib
-    return _built["lib"]
-
-
 def decode(data, backend="port", n_threads=0, samples=True):
     """The README loop; per frame (FrameId, samples or None, map bytes or None, stride_mb), and per NAL its return code.
     backend: "port" (CPU, with error maps), "gpu", or "oracle" (oracle/liboracle_dec.so: a backend without error maps)."""
-    lib = pkg.load() if backend == "gpu" else port_maps_lib() if backend == "port" else checkers.load("port")
+    lib = checkers.load("port") if backend == "oracle" else lib_of(backend)
     buf = ctypes.create_string_buffer(data, len(data) + 64)
     base = ctypes.addressof(buf); end = base + len(data)
     dec = lib.edge264_alloc(n_threads, None, None, 0, None, None, None)
@@ -204,13 +186,6 @@ def test_ramp_restatement_matches_the_reference_formula():
 
 
 # ---- 3. damaged streams ----
-def _damaged(workdir):
-    for name, w, h, args in DAMAGED_CASES:
-        src = open(make_stream(workdir, name, w, h, args), "rb").read()
-        for seed in range(25):
-            yield name, seed, damage(src, random.Random(seed * 7919 + len(src)))
-
-
 def test_damaged_streams_maps(workdir):
     """Values in 0..100, the same on a second run; where the samples agree across worker counts the maps agree too."""
     agree = total = 0
@@ -233,7 +208,7 @@ def test_damaged_streams_maps(workdir):
 
 def test_damaged_streams_keep_the_err_contract(workdir, monkeypatch):
     """E264_CHECK_RECORDS=1: every picture the parser submits keeps the record contract, err <= 100 included."""
-    lib = port_maps_lib()
+    lib = checkers.port_outputs_lib()
     monkeypatch.setenv("E264_CHECK_RECORDS", "1")
     for name, seed, data in _damaged(workdir):
         for t in (0, 1, 3):
@@ -266,46 +241,21 @@ def test_device_maps_match_port(workdir):
 
 
 # ---- 7. device memory output: the map stays in host memory ----
-_ALLOC = ctypes.CFUNCTYPE(None, ctypes.POINTER(ctypes.c_void_p), ctypes.c_uint, ctypes.POINTER(ctypes.c_void_p), ctypes.c_uint, ctypes.c_int, ctypes.c_void_p)
-_FREE = ctypes.CFUNCTYPE(None, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p)
-
-
 def _maps_with_device_samples(data):
     """Decode with alloc_cb handing out device memory (cudaMalloc); returns the maps only."""
-    cudart = ctypes.CDLL("libcudart.so.12") if os.path.exists("/usr/local/cuda/lib64/libcudart.so.12") else ctypes.CDLL(
-        os.path.join(os.path.dirname(__import__("torch").__file__), "lib", "libcudart.so.12"))
-    live = []
+    cudart = _cudart()
 
     def alloc(samples, size, mbs, mbs_size, err, arg):
         p = ctypes.c_void_p()
         assert cudart.cudaMalloc(ctypes.byref(p), ctypes.c_size_t(size)) == 0
-        live.append(p.value)
         samples[0] = p.value
     def free(samples, mbs, arg):
         cudart.cudaFree(ctypes.c_void_p(samples))
-    a, fr = _ALLOC(alloc), _FREE(free)
+    cbs = (_ALLOC(alloc), _FREE(free))
     lib = pkg.load()
-    buf = ctypes.create_string_buffer(data, len(data) + 64)
-    base = ctypes.addressof(buf); end = base + len(data)
-    dec = lib.edge264_alloc(0, None, None, 0, a, fr, None)
-    assert dec
-    nal = base + 3 + (1 if data[2] == 0 else 0)
-    maps, f = [], pkg.Edge264Frame()
-    while True:
-        sc = lib.edge264_find_start_code(nal, end, 0) if nal < end else end
-        before = len(maps)
-        res = lib.edge264_decode_NAL(dec, nal, sc, None, None)
-        while lib.edge264_get_frame(dec, ctypes.byref(f), 0) == 0:
-            maps.append((f.FrameId, pkg._frame_errors(f)))   # host memory: readable without a copy
-        if res == errno.ENOBUFS:
-            if len(maps) == before:
-                break
-            continue
-        if nal >= end:
-            break
-        nal = sc + 3 if sc + 3 < end else end
-    d = ctypes.c_void_p(dec)
-    lib.edge264_free(ctypes.byref(d))
+    dec, maps = new_decoder(lib, alloc=cbs), []
+    loop(lib, dec, data, lambda f: maps.append((f.FrameId, pkg._frame_errors(f))))   # host memory: readable without a copy
+    free_decoder(lib, dec)
     return maps
 
 

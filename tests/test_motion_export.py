@@ -1,37 +1,16 @@
 """The motion export (include/edge264_motion.h): per output frame, the vectors of every 4x4 block, the FrameId each 8x8
 block predicts from, the macroblock types and QP_Y, derived from the reconstruction records (e264_motion_kernel on the
 GPU).  CPU tests run the product's host sources over the plain-C restatement of the reconstruction and of the export
-(tests/native/port_motion_backend.c), bound into a library built here; the values are checked against the decoded pixels,
+(tests/native/port_outputs_backend.c), bound into a library built here; the values are checked against the decoded pixels,
 which are bit-exact with the reference decoder.  The GPU tests compare the device's export with that restatement."""
-import ctypes, errno, json, os, random, subprocess, sys, tempfile
+import ctypes, errno, json, os, subprocess, sys
 import numpy as np
 import pytest
 from conftest import ROOT, make_stream
-from test_robustness import CASES as DAMAGED_CASES, damage
+from api_helpers import lib_of, _ALLOC, _FREE, _cudart, _damaged
+from checkers import port_outputs_lib
 import edge264_b200 as pkg
 import checkers
-
-NATIVE = os.path.join(ROOT, "tests", "native")
-CSRC = os.path.join(ROOT, "edge264_b200", "csrc")
-_built = {}
-
-
-def port_motion_lib():
-    """The whole edge264 API on the CPU with error maps and the motion export."""
-    if "lib" not in _built:
-        path = os.path.join(tempfile.mkdtemp(prefix="e264motion"), "libport_motion.so")
-        src = [os.path.join(NATIVE, "port_motion_backend.c"), os.path.join(NATIVE, "port_error_map.c"), os.path.join(ROOT, "oracle", "port_recon.c"),
-               os.path.join(ROOT, "oracle", "record_check.c"), os.path.join(CSRC, "decoder.c"), os.path.join(CSRC, "slice_dec.c")]
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-w", "-o", path] + src + ["-pthread"], check=True)
-        lib = pkg.bind(path)
-        lib.e264_test_record_violations.restype = ctypes.c_int
-        lib.e264_test_last_violation.restype = ctypes.c_char_p
-        _built["lib"] = lib
-    return _built["lib"]
-
-
-def lib_of(backend):
-    return pkg.load() if backend == "gpu" else port_motion_lib()
 
 
 def decode(data, backend="port", n_threads=0, motion=True):
@@ -202,7 +181,7 @@ def _borrowed(lib, data):
 def test_borrowed_frames_keep_their_export(workdir):
     data = gen(workdir, *BREF)
     plain = {f[0]: f[5] for f in decode(data)[0]}
-    borrowed = _borrowed(port_motion_lib(), data)
+    borrowed = _borrowed(port_outputs_lib(), data)
     assert plain.keys() == borrowed.keys() and len(plain) == 30
     assert all(same_motion(plain[k], borrowed[k]) for k in plain)
 
@@ -212,7 +191,7 @@ def test_export_survives_flush(workdir):
     FrameIds apart (the numbering goes on across a flush, in the export's reference FrameIds as in the frames')."""
     data = gen(workdir, *BREF)
     fresh = [(f[0], f[5]) for f in decode(data)[0]]
-    lib = port_motion_lib()
+    lib = port_outputs_lib()
     buf = ctypes.create_string_buffer(data, len(data) + 64)
     base = ctypes.addressof(buf); end = base + len(data)
     dec = lib.edge264_alloc(0, None, None, 0, None, None, None)
@@ -252,17 +231,10 @@ def test_export_is_the_same_for_every_thread_count(workdir):
 
 
 # ---- 4. damaged streams ----
-def _damaged(workdir):
-    for name, w, h, args in DAMAGED_CASES:
-        src = gen(workdir, name, w, h, args)
-        for seed in range(25):
-            yield name, seed, damage(src, random.Random(seed * 7919 + len(src)))
-
-
 def test_damaged_streams_with_the_export(workdir, monkeypatch):
     """The record contract holds with the export on; samples and error maps are those of a decoder without it, and every
     FrameId the export names is one the decoder gave a picture."""
-    lib = port_motion_lib()
+    lib = port_outputs_lib()
     monkeypatch.setenv("E264_CHECK_RECORDS", "1")
     n = 0
     for name, seed, data in _damaged(workdir):
@@ -283,7 +255,7 @@ def test_damaged_streams_with_the_export(workdir, monkeypatch):
 # ---- 5. API ----
 def test_api_errors(workdir):
     data = gen(workdir, *BREF)
-    lib = port_motion_lib()
+    lib = port_outputs_lib()
     dec = lib.edge264_alloc(0, None, None, 0, None, None, None)
     buf = ctypes.create_string_buffer(data, len(data) + 64)
     base = ctypes.addressof(buf); end = base + len(data)
@@ -356,16 +328,6 @@ def test_device_export_matches_restatement(workdir):
 
 
 # ---- 7. the export where the samples are: device memory ----
-_ALLOC = ctypes.CFUNCTYPE(None, ctypes.POINTER(ctypes.c_void_p), ctypes.c_uint, ctypes.POINTER(ctypes.c_void_p), ctypes.c_uint, ctypes.c_int, ctypes.c_void_p)
-_FREE = ctypes.CFUNCTYPE(None, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p)
-
-
-def _cudart():
-    """The CUDA runtime the product library was linked with: once that is loaded, its soname resolves to it."""
-    pkg.load()
-    return ctypes.CDLL("libcudart.so.12")
-
-
 def motion_with_device_alloc(data):
     """Decode with an alloc_cb that hands out cudaMalloc memory: (FrameId, on_device, motion) per frame."""
     cudart = _cudart()

@@ -1,41 +1,22 @@
 """The packed output (include/edge264_packed.h): every output frame cropped, as I420 or NV12, box-downscaled by 1, 2, 4
 or 8 (e264_pack_kernel on the GPU).  The oracle of every case is a few lines of numpy over the frame's own full-size
 samples, which other tests pin bit for bit to the reference decoder.  CPU tests run the product's host sources over the
-plain-C restatement (tests/native/port_packed_backend.c on top of port_motion_backend.c), bound into a library built
-here; GPU tests run the product library."""
-import ctypes, errno, os, pickle, random, subprocess, sys, tempfile
+plain-C restatement (tests/native/port_outputs_backend.c), bound into a library built here; GPU tests run the product
+library."""
+import ctypes, errno, os, pickle, subprocess, sys
 import numpy as np
 import pytest
 from conftest import ROOT, STREAMS, DPB_STREAMS, make_stream
-from test_robustness import CASES as DAMAGED_CASES, damage
-from test_motion_export import port_motion_lib
+from test_robustness import CASES as DAMAGED_CASES
+from api_helpers import lib_of, new_decoder, free_decoder, first_frame, loop, with_alloc_cb, _libc, _cudart, _damaged
+from checkers import port_outputs_lib
 import edge264_b200 as pkg
 import checkers
 
-NATIVE = os.path.join(ROOT, "tests", "native")
 CSRC = os.path.join(ROOT, "edge264_b200", "csrc")
 I420, NV12 = pkg.PACKED_I420, pkg.PACKED_NV12
 MODES = [(f, k) for f in (I420, NV12) for k in range(4)]
 MODE_IDS = ["%s-k%d" % ("nv12" if f else "i420", k) for f, k in MODES]
-_built = {}
-
-
-def port_packed_lib():
-    """The whole edge264 API on the CPU with error maps, the motion export and the packed output."""
-    if "lib" not in _built:
-        path = os.path.join(tempfile.mkdtemp(prefix="e264packed"), "libport_packed.so")
-        src = [os.path.join(NATIVE, "port_packed_backend.c"), os.path.join(NATIVE, "port_motion_backend.c"), os.path.join(NATIVE, "port_error_map.c"),
-               os.path.join(ROOT, "oracle", "port_recon.c"), os.path.join(ROOT, "oracle", "record_check.c"), os.path.join(CSRC, "decoder.c"), os.path.join(CSRC, "slice_dec.c")]
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-w", "-o", path] + src + ["-pthread", "-Wl,--wrap=e264_default_backend"], check=True)
-        lib = pkg.bind(path)
-        lib.e264_test_record_violations.restype = ctypes.c_int
-        lib.e264_test_last_violation.restype = ctypes.c_char_p
-        _built["lib"] = lib
-    return _built["lib"]
-
-
-def lib_of(backend):
-    return pkg.load() if backend == "gpu" else port_packed_lib()
 
 
 def gen(workdir, name, w, h, args):
@@ -136,21 +117,10 @@ def test_oracle_is_not_a_cascade():
 
 
 # ---- 3. API contract ----
-def first_frame(lib, dec, data, buf):
-    base = ctypes.addressof(buf); end = base + len(data)
-    nal = base + 3 + (1 if data[2] == 0 else 0)
-    f = pkg.Edge264Frame()
-    while lib.edge264_get_frame(dec, ctypes.byref(f), 0) != 0:
-        sc = lib.edge264_find_start_code(nal, end, 0)
-        lib.edge264_decode_NAL(dec, nal, sc, None, None)
-        nal = sc + 3
-    return f
-
-
 def test_api_errors(workdir):
     data = gen(workdir, *BASIC[0])
     buf = ctypes.create_string_buffer(data, len(data) + 64)
-    lib = port_packed_lib()
+    lib = port_outputs_lib()
     assert lib.edge264_enable_packed(None, NV12, 0) == errno.EINVAL
     dec = lib.edge264_alloc(0, None, None, 0, None, None, None)
     for fmt, k in ((2, 0), (-1, 0), (NV12, 4), (I420, -1)):
@@ -206,51 +176,11 @@ def test_ctypes_layout_and_layout_arithmetic(tmp_path):
 BREF = ("pk_bref", 6, 5, "-n 30 -s 631 --gop IPB --bref --refs 3 --idr 17")
 
 
-def loop(lib, dec, data, on_frame, borrow=0, stop_after=None):
-    """The README loop over an already allocated decoder; on_frame(f) for every frame; returns the number of frames."""
-    buf = ctypes.create_string_buffer(data, len(data) + 64)
-    base = ctypes.addressof(buf); end = base + len(data)
-    nal, count = base + 3 + (1 if data[2] == 0 else 0), 0
-    while True:
-        sc = lib.edge264_find_start_code(nal, end, 0) if nal < end else end
-        before = count
-        res = lib.edge264_decode_NAL(dec, nal, sc, None, None)
-        while True:
-            f = pkg.Edge264Frame()
-            if lib.edge264_get_frame(dec, ctypes.byref(f), borrow):
-                break
-            count += 1
-            on_frame(f)
-        if res == errno.ENOBUFS:
-            if count == before:
-                break
-            continue
-        if nal >= end or (stop_after is not None and count >= stop_after):
-            break
-        nal = sc + 3 if sc + 3 < end else end
-    return count
-
-
-def new_decoder(lib, packed=None, motion=False, n_threads=0, alloc=(None, None)):
-    dec = lib.edge264_alloc(n_threads, None, None, 0, alloc[0], alloc[1], None)
-    assert dec
-    if motion:
-        assert lib.edge264_enable_motion(dec) == 0
-    if packed is not None:
-        assert lib.edge264_enable_packed(dec, *packed) == 0
-    return dec
-
-
-def free_decoder(lib, dec):
-    d = ctypes.c_void_p(dec)
-    lib.edge264_free(ctypes.byref(d))
-
-
 def test_borrowed_frames_keep_their_packed_picture(workdir):
     data = gen(workdir, *BREF)
-    lib = port_packed_lib()
+    lib = port_outputs_lib()
     plain = {f[0]: f[-1] for f in pkg.decode_bytes(data, lib, packed=(NV12, 1))[0]}
-    dec, held = new_decoder(lib, (NV12, 1)), []
+    dec, held = new_decoder(lib, packed=(NV12, 1)), []
     loop(lib, dec, data, held.append, borrow=1)
     got = {f.FrameId: pkg.frame_packed(lib, dec, f) for f in held}     # read after everything is decoded
     for f in held:
@@ -262,8 +192,8 @@ def test_borrowed_frames_keep_their_packed_picture(workdir):
 
 def test_buffers_are_reused_when_not_borrowed(workdir):
     data = gen(workdir, *BREF)
-    lib = port_packed_lib()
-    dec, ptrs = new_decoder(lib, (I420, 2)), set()
+    lib = port_outputs_lib()
+    dec, ptrs = new_decoder(lib, packed=(I420, 2)), set()
     def see(f):
         p = pkg.Edge264Packed()
         assert lib.edge264_get_packed(dec, ctypes.byref(f), ctypes.byref(p)) == 0
@@ -275,9 +205,9 @@ def test_buffers_are_reused_when_not_borrowed(workdir):
 
 def test_packed_output_survives_flush(workdir):
     data = gen(workdir, *BREF)
-    lib = port_packed_lib()
+    lib = port_outputs_lib()
     fresh = [f[-1] for f in pkg.decode_bytes(data, lib, packed=(NV12, 2))[0]]
-    dec, got = new_decoder(lib, (NV12, 2)), []
+    dec, got = new_decoder(lib, packed=(NV12, 2)), []
     loop(lib, dec, data, lambda f: None, stop_after=12)
     lib.edge264_flush(dec)
     loop(lib, dec, data, lambda f: got.append(pkg.frame_packed(lib, dec, f)))
@@ -289,51 +219,16 @@ def test_size_change_follows_each_frames_sps(workdir):
     a = gen(workdir, "pk_size_a", 5, 4, "-n 5 -s 641 --gop IPB --crop-right 6 --deblock 0")
     b = gen(workdir, "pk_size_b", 3, 6, "-n 5 -s 642 --gop IP --crop-left 2 --crop-bottom 10 --deblock 0")
     for fmt, k in ((NV12, 0), (I420, 1), (NV12, 3)):
-        frames, _ = pkg.decode_bytes(a + b + a, port_packed_lib(), packed=(fmt, k))
+        frames, _ = pkg.decode_bytes(a + b + a, port_outputs_lib(), packed=(fmt, k))
         assert [(f[1], f[2]) for f in frames] == [(74, 64)] * 5 + [(46, 86)] * 5 + [(74, 64)] * 5
         check(frames, fmt, k, "size change")
 
 
 # ---- 5. alloc_cb ----
-_ALLOC = ctypes.CFUNCTYPE(None, ctypes.POINTER(ctypes.c_void_p), ctypes.c_uint, ctypes.POINTER(ctypes.c_void_p), ctypes.c_uint, ctypes.c_int, ctypes.c_void_p)
-_FREE = ctypes.CFUNCTYPE(None, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p)
-
-
-def with_alloc_cb(lib, data, malloc, free, packed=None, motion=False):
-    """Decode through an alloc_cb / free_cb pair: (frames as (FrameId, w, h, packed, motion), [(samples_size, mbs_size)] calls)."""
-    live, calls = set(), []
-    def alloc(samples, size, mbs, mbs_size, err, arg):
-        p = malloc(size)
-        live.add(p); calls.append((size, mbs_size))
-        samples[0] = p
-    def release(samples, mbs, arg):
-        live.remove(samples)
-        free(samples)
-    cbs = (_ALLOC(alloc), _FREE(release))
-    dec, out = new_decoder(lib, packed, motion, alloc=cbs), []
-    def see(f):
-        out.append((f.FrameId, f.width_Y, f.height_Y, pkg.frame_packed(lib, dec, f) if packed is not None else None,
-                    pkg.frame_motion(lib, dec, f) if motion else None))
-        if packed is not None:
-            p = pkg.Edge264Packed()
-            assert lib.edge264_get_packed(dec, ctypes.byref(f), ctypes.byref(p)) == 0 and p.planes[0] in live
-    loop(lib, dec, data, see)
-    free_decoder(lib, dec)
-    assert not live, "buffers not returned through free_cb"
-    return out, calls
-
-
-def _libc():
-    libc = ctypes.CDLL(None)
-    libc.calloc.restype = ctypes.c_void_p; libc.calloc.argtypes = [ctypes.c_size_t, ctypes.c_size_t]
-    libc.free.argtypes = [ctypes.c_void_p]
-    return (lambda n: libc.calloc(1, n + 64)), libc.free
-
-
 def test_alloc_cb_gets_one_more_call_per_buffer(workdir):
     name, w, h, args = BREF
     data = gen(workdir, name, w, h, args)
-    lib = port_packed_lib()
+    lib = port_outputs_lib()
     malloc, free = _libc()
     ref = pkg.decode_bytes(data, lib, motion=True, packed=(NV12, 1))[0]
     _, off = with_alloc_cb(lib, data, malloc, free)
@@ -351,27 +246,20 @@ def test_alloc_cb_gets_one_more_call_per_buffer(workdir):
 # ---- 6. parse-ahead threads ----
 def test_packed_output_is_the_same_for_every_thread_count(workdir):
     data = gen(workdir, *BREF)
-    runs = [pkg.decode_bytes(data, port_packed_lib(), t, packed=(NV12, 1))[0] for t in (0, 1, 3)]
+    runs = [pkg.decode_bytes(data, port_outputs_lib(), t, packed=(NV12, 1))[0] for t in (0, 1, 3)]
     check(runs[0], NV12, 1)
     for r in runs[1:]:
         assert [f[:4] for f in r] == [f[:4] for f in runs[0]] and all(same_packed(a[-1], b[-1]) for a, b in zip(r, runs[0]))
 
 
 # ---- 7. damaged streams ----
-def _damaged(workdir, seeds=8):
-    for name, w, h, args in DAMAGED_CASES:
-        src = gen(workdir, name, w, h, args)
-        for seed in range(seeds):
-            yield name, seed, damage(src, random.Random(seed * 7919 + len(src)))
-
-
 def test_damaged_streams(workdir, monkeypatch):
     """The packed picture is a function of the samples, whatever they are; samples, error maps and return codes are those
     of a decoder without it, and the record contract holds."""
-    lib = port_packed_lib()
+    lib = port_outputs_lib()
     monkeypatch.setenv("E264_CHECK_RECORDS", "1")
     n = 0
-    for name, seed, data in _damaged(workdir):
+    for name, seed, data in _damaged(workdir, 8):
         fmt, k = MODES[(n * 3 + 1) % 8]
         on, codes_on = pkg.decode_bytes(data, lib, errors=True, packed=(fmt, k))
         off, codes_off = pkg.decode_bytes(data, lib, errors=True)
@@ -387,7 +275,7 @@ def test_not_enabled_is_a_decoder_without_the_feature(workdir):
     malloc, free = _libc()
     for s in (BREF, next(s for s in DPB_STREAMS if s[0] == "crop_rect")):
         data = gen(workdir, *s)
-        new, old = port_packed_lib(), port_motion_lib()     # the second library's backend has no packed output at all
+        new, old = port_outputs_lib(), checkers.load("port")     # the second library's backend has no packed output at all
         assert pkg.decode_bytes(data, new, errors=True) == pkg.decode_bytes(data, old, errors=True)
         a, calls_new = with_alloc_cb(new, data, malloc, free)
         b, calls_old = with_alloc_cb(old, data, malloc, free)
@@ -418,11 +306,6 @@ def test_device_large_pictures(workdir, name, w, h):
 
 
 # ---- 10. the packed picture where the samples are: device memory ----
-def _cudart():
-    pkg.load()
-    return ctypes.CDLL("libcudart.so.12")
-
-
 # the samples are device memory too: only the packed picture is read (through torch)
 _SUB = """
 import sys, ctypes, errno, pickle
@@ -479,7 +362,7 @@ def test_device_matches_restatement_on_damaged_streams_and_with_threads(workdir)
     for name, seed, data in _damaged(workdir, 6):
         fmt, k = MODES[(n * 3 + 2) % 8]
         g, gc = pkg.decode_bytes(data, pkg.load(), errors=True, packed=(fmt, k))
-        p, pc = pkg.decode_bytes(data, port_packed_lib(), errors=True, packed=(fmt, k))
+        p, pc = pkg.decode_bytes(data, port_outputs_lib(), errors=True, packed=(fmt, k))
         assert gc == pc and [f[:5] for f in g] == [f[:5] for f in p], (name, seed)
         assert all(same_packed(a[-1], b[-1]) for a, b in zip(g, p)), (name, seed)
         n += 1
@@ -487,7 +370,7 @@ def test_device_matches_restatement_on_damaged_streams_and_with_threads(workdir)
     for t in (1, 3):
         for fmt, k in ((NV12, 1), (I420, 3)):
             g = pkg.decode_bytes(data, pkg.load(), t, motion=True, packed=(fmt, k))[0]
-            p = pkg.decode_bytes(data, port_packed_lib(), t, motion=True, packed=(fmt, k))[0]
+            p = pkg.decode_bytes(data, port_outputs_lib(), t, motion=True, packed=(fmt, k))[0]
             assert [f[:4] for f in g] == [f[:4] for f in p] and all(same_packed(a[-1], b[-1]) for a, b in zip(g, p))
             assert all(np.array_equal(a[-2][m], b[-2][m]) for a, b in zip(g, p) for m in b[-2])
 
@@ -497,7 +380,7 @@ def _stats(data, packed, touch=True):
     lib = pkg.load()
     lib.e264b_of_decoder.restype = ctypes.c_void_p; lib.e264b_of_decoder.argtypes = [ctypes.c_void_p]
     lib.e264b_stats.argtypes = [ctypes.c_void_p] + [ctypes.POINTER(ctypes.c_uint64)] * 3
-    dec = new_decoder(lib, packed)
+    dec = new_decoder(lib, packed=packed)
     if packed is None and touch:      # refused calls leave the decoder as it was
         assert lib.edge264_enable_packed(dec, 7, 0) == errno.EINVAL
     frames = []

@@ -2,42 +2,23 @@
 sums of squares of every coded macroblock (e264_picstats_kernel on the GPU).  The oracle is numpy over the frame's coded
 planes, read through Edge264Frame.samples[], frame_crop_offsets and the strides with ctypes (not through the cropped bytes
 decode_bytes returns), which other tests pin bit for bit to the reference decoder.  CPU tests run the product's host
-sources over the plain-C restatement (tests/native/port_picstats_backend.c, on top of port_resized_backend.c), bound into
-a library built here; GPU tests compare the product library with it byte for byte."""
-import ctypes, errno, os, pickle, subprocess, sys, tempfile, threading
+sources over the plain-C restatement (tests/native/port_outputs_backend.c), bound into a library built here; GPU tests
+compare the product library with it byte for byte."""
+import ctypes, errno, os, pickle, subprocess, sys, threading
 import numpy as np
 import pytest
 from conftest import ROOT, STREAMS, DPB_STREAMS, make_stream
 from test_limits import LIMITS
-from test_motion_export import port_motion_lib
-from test_packed_output import BREF, P1080, loop, free_decoder, first_frame, _libc, _ALLOC, _FREE, _damaged, _cudart
+from test_packed_output import BREF, P1080
 from test_luma_only import STORED
+from api_helpers import new_decoder, free_decoder, first_frame, loop, with_alloc_cb, _libc, _ALLOC, _FREE, _cudart, _damaged
+from checkers import port_outputs_lib
 import edge264_b200 as pkg
+import checkers
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 from picstats_cost import constant_stream   # noqa: E402
 
-NATIVE = os.path.join(ROOT, "tests", "native")
 CSRC = os.path.join(ROOT, "edge264_b200", "csrc")
-_built = {}
-
-
-def port_picstats_lib():
-    """The whole edge264 API on the CPU with error maps, the motion export, the packed and resized output and the
-    statistics.  port_resized_backend.c also defines __wrap_e264_default_backend: its object gets that symbol renamed to
-    port_resized_default_backend, the table port_picstats_backend.c extends."""
-    if "lib" not in _built:
-        tmp = tempfile.mkdtemp(prefix="e264picstats")
-        obj, path = os.path.join(tmp, "port_resized_backend.o"), os.path.join(tmp, "libport_picstats.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-w", "-c", "-o", obj, os.path.join(NATIVE, "port_resized_backend.c")], check=True)
-        subprocess.run(["objcopy", "--redefine-sym", "__wrap_e264_default_backend=port_resized_default_backend", obj], check=True)
-        src = [os.path.join(NATIVE, "port_picstats_backend.c"), obj, os.path.join(NATIVE, "port_motion_backend.c"), os.path.join(NATIVE, "port_error_map.c"),
-               os.path.join(ROOT, "oracle", "port_recon.c"), os.path.join(ROOT, "oracle", "record_check.c"), os.path.join(CSRC, "decoder.c"), os.path.join(CSRC, "slice_dec.c")]
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-w", "-o", path] + src + ["-pthread", "-Wl,--wrap=e264_default_backend"], check=True)
-        lib = pkg.bind(path)
-        lib.e264_test_record_violations.restype = ctypes.c_int
-        lib.e264_test_last_violation.restype = ctypes.c_char_p
-        _built["lib"] = lib
-    return _built["lib"]
 
 
 def _data(workdir, s):
@@ -94,24 +75,10 @@ def check(got, f, want, label):
         assert int((np.arange(256) * got["hist"][0].astype(np.int64)).sum()) == int(got["sum"][0].astype(np.int64).sum()), label
 
 
-def new_decoder(lib, n_threads=0, picstats=True, luma_only=False, skip=pkg.SKIP_NONE, motion=False, alloc=(None, None)):
-    dec = lib.edge264_alloc(n_threads, None, None, 0, alloc[0], alloc[1], None)
-    assert dec
-    if motion:
-        assert lib.edge264_enable_motion(dec) == 0
-    if picstats:
-        assert lib.edge264_enable_picstats(dec) == 0
-    if luma_only:
-        assert lib.edge264_enable_luma_only(dec) == 0
-    if skip != pkg.SKIP_NONE:
-        assert lib.edge264_set_skip(dec, skip) == 0
-    return dec
-
-
 def run(lib, data, label="", with_oracle=True, **kw):
     """Decode with the statistics on; every frame checked against the oracle (host memory).  Returns
     [(FrameId, stats)]."""
-    dec, out = new_decoder(lib, **kw), []
+    dec, out = new_decoder(lib, picstats=True, **kw), []
     def see(f):
         got = pkg.frame_picstats(lib, dec, f)
         if with_oracle:
@@ -138,7 +105,7 @@ IDS = [_id(s) for s in ALL]
 # ---- 1. CPU: the restatement against numpy ----
 @pytest.mark.parametrize("stream", ALL, ids=IDS)
 def test_port_matches_the_definition_with_every_thread_count(workdir, stream):
-    data, lib = _data(workdir, stream), port_picstats_lib()
+    data, lib = _data(workdir, stream), port_outputs_lib()
     runs = [sorted(run(lib, data, "%s t%d" % (_id(stream), t), n_threads=t), key=lambda x: x[0]) for t in (0, 1, 3)]   # by FrameId: the
     assert runs[0]                                                                                                         # output order may differ
     same_runs(runs[0], runs[1], _id(stream)); same_runs(runs[0], runs[2], _id(stream))
@@ -148,8 +115,8 @@ def test_streams_cover_cropping_and_shapes(workdir):
     """crop_rect crops all four sides, inside macroblocks; zero-cropping.264, wide_256x2 and ragged_1x1_intra are there."""
     ids = set(IDS)
     assert {"crop_rect", "wide_256x2", "ragged_1x1_intra", "zero-cropping.264"} <= ids and len(STORED) >= 7
-    lib, seen = port_picstats_lib(), []
-    dec = new_decoder(lib)
+    lib, seen = port_outputs_lib(), []
+    dec = new_decoder(lib, picstats=True)
     loop(lib, dec, _data(workdir, next(s for s in DPB_STREAMS if s[0] == "crop_rect")), lambda f: seen.append(tuple(f.frame_crop_offsets)))
     free_decoder(lib, dec)
     assert set(seen) == {(8, 6, 4, 10)}
@@ -157,7 +124,7 @@ def test_streams_cover_cropping_and_shapes(workdir):
 
 def test_every_other_output_is_unchanged(workdir):
     """Samples, FrameIds, return codes, error maps, motion export, packed and resized output equal a decode without it."""
-    lib = port_picstats_lib()
+    lib = port_outputs_lib()
     for s in (BREF, next(x for x in DPB_STREAMS if x[0] == "crop_rect"), next(x for x in STREAMS if x[0] == "b_explicit")):
         data = _data(workdir, s)
         for t in (0, 3):
@@ -174,10 +141,10 @@ def test_every_other_output_is_unchanged(workdir):
 @pytest.mark.parametrize("stream", GENERATED, ids=[s[0] for s in GENERATED])
 def test_luma_only(workdir, stream):
     """Luma statistics equal the full decode's; chroma is a plane of 128."""
-    data, lib, s = _data(workdir, stream), port_picstats_lib(), stream[0]
+    data, lib, s = _data(workdir, stream), port_outputs_lib(), stream[0]
     full, luma = run(lib, data, s), run(lib, data, s + " luma", luma_only=True)
     assert [x[0] for x in full] == [x[0] for x in luma]
-    dec = new_decoder(lib, luma_only=True)
+    dec = new_decoder(lib, picstats=True, luma_only=True)
     sizes = []
     loop(lib, dec, data, lambda f: sizes.append(f.width_C * f.height_C))
     free_decoder(lib, dec)
@@ -191,7 +158,7 @@ def test_luma_only(workdir, stream):
 @pytest.mark.parametrize("skip", [pkg.SKIP_NONREF, pkg.SKIP_NONKEY], ids=["nonref", "nonkey"])
 def test_skip_modes(workdir, skip):
     """Each output frame's statistics are those of the same FrameId in the full decode."""
-    lib, n = port_picstats_lib(), 0
+    lib, n = port_outputs_lib(), 0
     for s in GENERATED:
         data = _data(workdir, s)
         full = dict((i, st) for i, st in run(lib, data, s[0]))
@@ -204,10 +171,10 @@ def test_skip_modes(workdir, skip):
 # ---- 2. lifetimes and buffers ----
 def test_borrowed_frames_and_flush(workdir):
     data = _data(workdir, BREF)
-    lib = port_picstats_lib()
+    lib = port_outputs_lib()
     order = run(lib, data, "bref")
     fresh = dict(order)
-    dec, held = new_decoder(lib), []
+    dec, held = new_decoder(lib, picstats=True), []
     loop(lib, dec, data, held.append, borrow=1)
     got = {f.FrameId: pkg.frame_picstats(lib, dec, f) for f in held}   # read after everything is decoded
     for f in held:
@@ -215,7 +182,7 @@ def test_borrowed_frames_and_flush(workdir):
     assert lib.edge264_get_picstats(dec, ctypes.byref(held[0]), ctypes.byref(pkg.Edge264PicStats())) == errno.EINVAL
     free_decoder(lib, dec)
     assert got.keys() == fresh.keys() and len(got) == 30 and all(same_stats(got[i], fresh[i]) for i in got)
-    dec, after = new_decoder(lib), []
+    dec, after = new_decoder(lib, picstats=True), []
     loop(lib, dec, data, lambda f: None, stop_after=12)
     lib.edge264_flush(dec)
     loop(lib, dec, data, lambda f: after.append((f.FrameId, pkg.frame_picstats(lib, dec, f))))
@@ -226,57 +193,32 @@ def test_borrowed_frames_and_flush(workdir):
 def test_size_change(workdir):
     a = _data(workdir, ("pk_size_a", 5, 4, "-n 5 -s 641 --gop IPB --crop-right 6 --deblock 0"))
     b = _data(workdir, ("pk_size_b", 3, 6, "-n 5 -s 642 --gop IP --crop-left 2 --crop-bottom 10 --deblock 0"))
-    got = run(port_picstats_lib(), a + b + a, "size change")
+    got = run(port_outputs_lib(), a + b + a, "size change")
     assert [st["sum"].shape for _, st in got] == [(3, 4, 5)] * 5 + [(3, 6, 3)] * 5 + [(3, 4, 5)] * 5
-
-
-def with_alloc_cb(lib, data, malloc, free, **kw):
-    """Decode through an alloc_cb / free_cb pair: ([(FrameId, stats)], [(samples_size, mbs_size)] calls)."""
-    live, calls = set(), []
-    def alloc(samples, size, mbs, mbs_size, err, arg):
-        p = malloc(size)
-        live.add(p); calls.append((size, mbs_size))
-        samples[0] = p
-    def release(samples, mbs, arg):
-        live.remove(samples)
-        free(samples)
-    cbs = (_ALLOC(alloc), _FREE(release))
-    dec, out = new_decoder(lib, alloc=cbs, **kw), []
-    def see(f):
-        if kw.get("picstats", True):
-            s = pkg.Edge264PicStats()
-            assert lib.edge264_get_picstats(dec, ctypes.byref(f), ctypes.byref(s)) == 0 and ctypes.cast(s.hist, ctypes.c_void_p).value in live
-            out.append((f.FrameId, pkg.frame_picstats(lib, dec, f)))
-        else:
-            out.append((f.FrameId, None))
-    loop(lib, dec, data, see)
-    free_decoder(lib, dec)
-    assert not live, "buffers not returned through free_cb"
-    return out, calls
 
 
 def test_alloc_cb_gets_one_more_call_per_buffer(workdir):
     name, w, h, args = BREF
     data = _data(workdir, BREF)
-    lib = port_picstats_lib()
+    lib = port_outputs_lib()
     malloc, free = _libc()
     ref = run(lib, data, "bref")
     _, off = with_alloc_cb(lib, data, malloc, free, picstats=False)
-    on, calls = with_alloc_cb(lib, data, malloc, free)
-    both, calls2 = with_alloc_cb(lib, data, malloc, free, motion=True)
+    on, calls = with_alloc_cb(lib, data, malloc, free, picstats=True)
+    both, calls2 = with_alloc_cb(lib, data, malloc, free, picstats=True, motion=True)
     size = 3072 + 24 * w * h
     assert all(m for _, m in off)
     assert calls == [c for s in off for c in (s, (size, 0))]
     assert calls2 == [c for s in off for c in (s, (162 * w * h, 0), (size, 0))]
     for got in (on, both):
-        same_runs(got, ref, "alloc_cb")
+        same_runs([(g[0], g[5]) for g in got], ref, "alloc_cb")
 
 
 def test_alloc_cb_order_with_packed_output(workdir):
     """The statistics' buffer is asked for after the packed one."""
     name, w, h, args = BREF
     data = _data(workdir, BREF)
-    lib = port_picstats_lib()
+    lib = port_outputs_lib()
     malloc, free = _libc()
     live, calls = set(), []
     def alloc(samples, size, mbs, mbs_size, err, arg):
@@ -284,7 +226,7 @@ def test_alloc_cb_order_with_packed_output(workdir):
     def release(samples, mbs, arg):
         live.remove(samples); free(samples)
     cbs = (_ALLOC(alloc), _FREE(release))
-    dec = new_decoder(lib, alloc=cbs)
+    dec = new_decoder(lib, picstats=True, alloc=cbs)
     assert lib.edge264_enable_packed(dec, pkg.PACKED_NV12, 3) == 0
     loop(lib, dec, data, lambda f: None)
     free_decoder(lib, dec)
@@ -296,10 +238,10 @@ def test_alloc_cb_order_with_packed_output(workdir):
 def test_damaged_streams(workdir, monkeypatch):
     """The statistics are a function of the samples, whatever they are; samples, error maps and return codes are those of
     a decoder without them, and the record contract holds."""
-    lib = port_picstats_lib()
+    lib = port_outputs_lib()
     monkeypatch.setenv("E264_CHECK_RECORDS", "1")
     n = 0
-    for name, seed, data in _damaged(workdir):
+    for name, seed, data in _damaged(workdir, 8):
         on, codes_on = pkg.decode_bytes(data, lib, errors=True, picstats=True)
         off, codes_off = pkg.decode_bytes(data, lib, errors=True)
         assert lib.e264_test_record_violations() == 0, "%s seed %d: %s" % (name, seed, lib.e264_test_last_violation())
@@ -313,7 +255,7 @@ def test_damaged_streams(workdir, monkeypatch):
 def test_api_codes(workdir):
     data = _data(workdir, STREAMS[0])
     buf = ctypes.create_string_buffer(data, len(data) + 64)
-    lib = port_picstats_lib()
+    lib = port_outputs_lib()
     assert lib.edge264_enable_picstats(None) == errno.EINVAL
     dec = lib.edge264_alloc(0, None, None, 0, None, None, None)
     f = first_frame(lib, dec, data, buf)
@@ -331,7 +273,7 @@ def test_api_codes(workdir):
     assert lib.edge264_get_picstats(dec, ctypes.byref(f), ctypes.byref(s)) == errno.EINVAL   # no longer held
     free_decoder(lib, dec)
     # a backend without submit_outputs
-    plain = port_motion_lib()
+    plain = checkers.load("port")
     dec = plain.edge264_alloc(0, None, None, 0, None, None, None)
     assert plain.edge264_enable_picstats(dec) == errno.ENOTSUP
     free_decoder(plain, dec)
@@ -358,7 +300,7 @@ def test_not_enabled_is_a_decoder_without_the_feature(workdir):
     malloc, free = _libc()
     for s in (BREF, next(x for x in DPB_STREAMS if x[0] == "crop_rect")):
         data = _data(workdir, s)
-        new, old = port_picstats_lib(), port_motion_lib()
+        new, old = port_outputs_lib(), checkers.load("port")
         assert pkg.decode_bytes(data, new, errors=True) == pkg.decode_bytes(data, old, errors=True)
         a, calls_new = with_alloc_cb(new, data, malloc, free, picstats=False)
         b, calls_old = with_alloc_cb(old, data, malloc, free, picstats=False)
@@ -373,7 +315,7 @@ LARGE = [("ps_1088p", 120, 68, "-n 2 -s 682 --gop IP --density 20 --deblock 0"),
 
 def same_as_restatement(data, label, n_threads=0, **kw):
     g = run(pkg.load(), data, label + " gpu", n_threads=n_threads, **kw)
-    p = run(port_picstats_lib(), data, label + " port", n_threads=n_threads, **kw)
+    p = run(port_outputs_lib(), data, label + " port", n_threads=n_threads, **kw)
     same_runs(g, p, label)
     for _, st in g:
         assert st["on_device"] == 0
@@ -390,7 +332,7 @@ def test_device_matches_restatement(workdir, stream):
 
 
 def test_constant_stream_decodes_to_constant_planes():
-    lib = port_picstats_lib()
+    lib = port_outputs_lib()
     for w, h, crop, v in CONSTANT:
         for luma_only in (False, True):
             frames, codes = pkg.decode_bytes(constant_stream(w, h, 3, v, crop), lib, luma_only=luma_only, picstats=True)
@@ -428,7 +370,7 @@ def test_device_decoders_in_parallel(workdir):
     """Decoders on 8 host threads at once, every other one luma-only, match the restatement."""
     streams = [s for s in GENERATED if s[0] in ("crop_rect", "b_explicit", "pb_intra_heavy", "wide_33x2", "bref_spatial", "p_refs_wp", "ps_update", "b_cavlc_all")]
     datas = [_data(workdir, s) for s in streams]
-    want = [run(port_picstats_lib(), d, s[0], luma_only=bool(i % 2)) for i, (s, d) in enumerate(zip(streams, datas))]
+    want = [run(port_outputs_lib(), d, s[0], luma_only=bool(i % 2)) for i, (s, d) in enumerate(zip(streams, datas))]
     got, errs = [None] * len(datas), []
     def work(i):
         try:
@@ -481,7 +423,7 @@ def test_device_memory_output(workdir):
         p = ctypes.c_void_p()
         assert cudart.cudaMalloc(ctypes.byref(p), n) == 0
         return p.value
-    got, _ = with_alloc_cb(pkg.load(), data, dmalloc, cudart.cudaFree)
+    got = [(g[0], g[5]) for g in with_alloc_cb(pkg.load(), data, dmalloc, cudart.cudaFree, picstats=True)[0]]
     assert all(st["on_device"] == 1 for _, st in got)
     same_runs(got, host, "alloc_cb device memory")
     src, out = os.path.join(workdir, "ps_dev.264"), os.path.join(workdir, "ps_dev.pkl")

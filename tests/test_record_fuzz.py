@@ -8,10 +8,10 @@ vectors at the picture borders, every boundary strength, up to 64 slices, every 
 intra kernels — and compares the device's frames with oracle/port_recon.c byte for byte.  Every such picture keeps the
 record contract first: the device is only ever given records the parser could emit, and the parser keeps that
 contract even on damaged streams."""
-import os, random, re, subprocess
+import os, re, subprocess
 import pytest
 from conftest import ROOT, STREAMS, DPB_STREAMS, make_stream
-from test_robustness import CASES as DAMAGED_CASES, damage
+from api_helpers import _damaged
 
 FUZZ_SRC = [os.path.join(ROOT, "tests", "native", "record_fuzz.c"), os.path.join(ROOT, "oracle", "port_recon.c"), os.path.join(ROOT, "oracle", "record_check.c")]
 # seed k draws geometry k % 18 of the driver's list (1x1 ... 120x68, 256x2): two rounds cover every geometry twice
@@ -64,14 +64,6 @@ def test_stored_streams_keep_the_contract():
     for p in paths:
         code, why = _check_records(p)
         assert code == 0, (os.path.basename(p), why)
-
-
-def _damaged(workdir):
-    """The 75 damaged streams of test_robustness.py, same mutations and seeds."""
-    for name, w, h, args in DAMAGED_CASES:
-        src = open(make_stream(workdir, name, w, h, args), "rb").read()
-        for seed in range(25):
-            yield name, seed, damage(src, random.Random(seed * 7919 + len(src)))
 
 
 def test_damaged_streams_keep_the_contract(workdir):

@@ -2,40 +2,20 @@
 resampled to any size by exact area averaging (e264_resize_kernel on the GPU).  The oracle is a few lines of numpy over
 the frame's own full-size samples, which other tests pin bit for bit to the reference decoder: the integer overlap
 matrices A_v (t_h x s_h) and A_h (t_w x s_w), N = A_v P A_h^T, out = (2 N + D) // 2D.  CPU tests run the product's host
-sources over the plain-C restatement (tests/native/port_resized_backend.c, on top of port_packed_backend.c and
-port_motion_backend.c), bound into a library built here; GPU tests compare the product library with it byte for byte."""
-import ctypes, errno, os, pickle, random, subprocess, sys, tempfile
+sources over the plain-C restatement (tests/native/port_outputs_backend.c), bound into a library built here; GPU tests
+compare the product library with it byte for byte."""
+import ctypes, errno, os, pickle, random, subprocess, sys
 import numpy as np
 import pytest
 from conftest import ROOT, DPB_STREAMS
-from test_motion_export import port_motion_lib
-from test_packed_output import (BASIC, EDGES, P1080, GPU_WIDTHS, BREF, gen, first_frame, loop, free_decoder, same_packed, layout_bytes,
-                                port_packed_lib, _libc, _ALLOC, _FREE, _damaged, _cudart)
+from test_packed_output import BASIC, EDGES, P1080, GPU_WIDTHS, BREF, gen, same_packed, layout_bytes
+from api_helpers import lib_of, new_decoder, free_decoder, first_frame, loop, with_alloc_cb, _libc, _cudart, _damaged
+from checkers import port_outputs_lib
 import edge264_b200 as pkg
 import checkers
 
-NATIVE = os.path.join(ROOT, "tests", "native")
 CSRC = os.path.join(ROOT, "edge264_b200", "csrc")
 I420, NV12 = pkg.PACKED_I420, pkg.PACKED_NV12
-_built = {}
-
-
-def port_resized_lib():
-    """The whole edge264 API on the CPU with error maps, the motion export, the packed and the resized output."""
-    if "lib" not in _built:
-        path = os.path.join(tempfile.mkdtemp(prefix="e264resized"), "libport_resized.so")
-        src = [os.path.join(NATIVE, "port_resized_backend.c"), os.path.join(NATIVE, "port_motion_backend.c"), os.path.join(NATIVE, "port_error_map.c"),
-               os.path.join(ROOT, "oracle", "port_recon.c"), os.path.join(ROOT, "oracle", "record_check.c"), os.path.join(CSRC, "decoder.c"), os.path.join(CSRC, "slice_dec.c")]
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-w", "-o", path] + src + ["-pthread", "-Wl,--wrap=e264_default_backend"], check=True)
-        lib = pkg.bind(path)
-        lib.e264_test_record_violations.restype = ctypes.c_int
-        lib.e264_test_last_violation.restype = ctypes.c_char_p
-        _built["lib"] = lib
-    return _built["lib"]
-
-
-def lib_of(backend):
-    return pkg.load() if backend == "gpu" else port_resized_lib()
 
 
 # ---- the definition, in numpy ----
@@ -130,7 +110,7 @@ def power_of_two_ratios(workdir, stream, backend):
             if (W >> k) % 2 or (H >> k) % 2 or (W >> k) << k != W or (H >> k) << k != H:
                 continue
             a = pkg.decode_bytes(data, lib, resized=(fmt, W >> k, H >> k))[0]
-            b = pkg.decode_bytes(data, lib if backend == "gpu" else port_packed_lib(), packed=(fmt, k))[0]
+            b = pkg.decode_bytes(data, lib, packed=(fmt, k))[0]
             assert all(x[-1]["log2_scale"] == -1 and y[-1]["log2_scale"] == k for x, y in zip(a, b))
             assert all(all(np.array_equal(x[-1][m], y[-1][m]) for m in y[-1] if m not in ("log2_scale", "on_device")) for x, y in zip(a, b))
             n += 1
@@ -177,7 +157,7 @@ def test_rounding_helper_against_python_integers(tmp_path):
 def test_api_errors_and_replacement(workdir):
     data = gen(workdir, *BASIC[0])
     buf = ctypes.create_string_buffer(data, len(data) + 64)
-    lib = port_resized_lib()
+    lib = port_outputs_lib()
     assert lib.edge264_enable_resized(None, NV12, 64, 64) == errno.EINVAL
     dec = lib.edge264_alloc(0, None, None, 0, None, None, None)
     for args in ((2, 64, 64), (-1, 64, 64), (NV12, 63, 64), (I420, 64, 35), (NV12, 0, 0), (NV12, 16386, 64), (I420, 64, 16386), (NV12, -2, 64), (NV12, 64, -2)):
@@ -224,29 +204,19 @@ def test_size_change(workdir):
     a = gen(workdir, "pk_size_a", 5, 4, "-n 5 -s 641 --gop IPB --crop-right 6 --deblock 0")
     b = gen(workdir, "pk_size_b", 3, 6, "-n 5 -s 642 --gop IP --crop-left 2 --crop-bottom 10 --deblock 0")
     for fmt, tw, th, shapes in ((NV12, 64, 48, [(64, 48)] * 3), (I420, 40, 0, [(40, 34), (40, 74), (40, 34)]), (NV12, 0, 30, [(34, 30), (16, 30), (34, 30)])):
-        frames, _ = pkg.decode_bytes(a + b + a, port_resized_lib(), resized=(fmt, tw, th))
+        frames, _ = pkg.decode_bytes(a + b + a, port_outputs_lib(), resized=(fmt, tw, th))
         assert [(f[1], f[2]) for f in frames] == [(74, 64)] * 5 + [(46, 86)] * 5 + [(74, 64)] * 5
         assert [(f[-1]["y"].shape[1], f[-1]["y"].shape[0]) for f in frames] == [s for s in shapes for _ in range(5)]
         check(frames, fmt, tw, th, "size change")
 
 
-def new_decoder(lib, resized=None, motion=False, n_threads=0, alloc=(None, None)):
-    dec = lib.edge264_alloc(n_threads, None, None, 0, alloc[0], alloc[1], None)
-    assert dec
-    if motion:
-        assert lib.edge264_enable_motion(dec) == 0
-    if resized is not None:
-        assert lib.edge264_enable_resized(dec, *resized) == 0
-    return dec
-
-
 def test_borrowed_frames_and_flush(workdir):
     data = gen(workdir, *BREF)
-    lib = port_resized_lib()
+    lib = port_outputs_lib()
     fresh = pkg.decode_bytes(data, lib, resized=(NV12, 30, 22))[0]
     check(fresh, NV12, 30, 22)
     plain = {f[0]: f[-1] for f in fresh}
-    dec, held = new_decoder(lib, (NV12, 30, 22)), []
+    dec, held = new_decoder(lib, resized=(NV12, 30, 22)), []
     loop(lib, dec, data, held.append, borrow=1)
     got = {f.FrameId: pkg.frame_packed(lib, dec, f) for f in held}     # read after everything is decoded
     for f in held:
@@ -254,7 +224,7 @@ def test_borrowed_frames_and_flush(workdir):
     assert lib.edge264_get_packed(dec, ctypes.byref(held[0]), ctypes.byref(pkg.Edge264Packed())) == errno.EINVAL
     free_decoder(lib, dec)
     assert plain.keys() == got.keys() and len(plain) == 30 and all(same_packed(plain[i], got[i]) for i in plain)
-    dec, got = new_decoder(lib, (NV12, 30, 22)), []
+    dec, got = new_decoder(lib, resized=(NV12, 30, 22)), []
     loop(lib, dec, data, lambda f: None, stop_after=12)
     lib.edge264_flush(dec)
     loop(lib, dec, data, lambda f: got.append(pkg.frame_packed(lib, dec, f)))
@@ -263,34 +233,10 @@ def test_borrowed_frames_and_flush(workdir):
 
 
 # ---- 4. alloc_cb ----
-def with_alloc_cb(lib, data, malloc, free, resized=None, motion=False):
-    """Decode through an alloc_cb / free_cb pair: (frames as (FrameId, w, h, packed, motion), [(samples_size, mbs_size)] calls)."""
-    live, calls = set(), []
-    def alloc(samples, size, mbs, mbs_size, err, arg):
-        p = malloc(size)
-        live.add(p); calls.append((size, mbs_size))
-        samples[0] = p
-    def release(samples, mbs, arg):
-        live.remove(samples)
-        free(samples)
-    cbs = (_ALLOC(alloc), _FREE(release))
-    dec, out = new_decoder(lib, resized, motion, alloc=cbs), []
-    def see(f):
-        out.append((f.FrameId, f.width_Y, f.height_Y, pkg.frame_packed(lib, dec, f) if resized is not None else None,
-                    pkg.frame_motion(lib, dec, f) if motion else None))
-        if resized is not None:
-            p = pkg.Edge264Packed()
-            assert lib.edge264_get_packed(dec, ctypes.byref(f), ctypes.byref(p)) == 0 and p.planes[0] in live
-    loop(lib, dec, data, see)
-    free_decoder(lib, dec)
-    assert not live, "buffers not returned through free_cb"
-    return out, calls
-
-
 def test_alloc_cb_gets_one_more_call_per_buffer(workdir):
     name, w, h, args = BREF
     data = gen(workdir, name, w, h, args)
-    lib = port_resized_lib()
+    lib = port_outputs_lib()
     malloc, free = _libc()
     ref = pkg.decode_bytes(data, lib, motion=True, resized=(I420, 50, 0))[0]
     _, off = with_alloc_cb(lib, data, malloc, free)
@@ -308,7 +254,7 @@ def test_alloc_cb_gets_one_more_call_per_buffer(workdir):
 # ---- 5. threads, damaged streams, off ----
 def test_resized_output_is_the_same_for_every_thread_count(workdir):
     data = gen(workdir, *BREF)
-    runs = [pkg.decode_bytes(data, port_resized_lib(), t, resized=(NV12, 38, 26))[0] for t in (0, 1, 3)]
+    runs = [pkg.decode_bytes(data, port_outputs_lib(), t, resized=(NV12, 38, 26))[0] for t in (0, 1, 3)]
     check(runs[0], NV12, 38, 26)
     for r in runs[1:]:
         assert [f[:4] for f in r] == [f[:4] for f in runs[0]] and all(same_packed(a[-1], b[-1]) for a, b in zip(r, runs[0]))
@@ -320,7 +266,7 @@ DAMAGED_TARGETS = [(I420, 22, 14), (NV12, 224, 224), (NV12, 0, 10), (I420, 6, 0)
 def test_damaged_streams(workdir, monkeypatch):
     """The resized picture is a function of the samples, whatever they are; samples, error maps and return codes are
     those of a decoder without it, and the record contract holds."""
-    lib = port_resized_lib()
+    lib = port_outputs_lib()
     monkeypatch.setenv("E264_CHECK_RECORDS", "1")
     for n, (name, seed, data) in enumerate(_damaged(workdir, 4)):
         fmt, tw, th = DAMAGED_TARGETS[n % 4]
@@ -335,7 +281,7 @@ def test_not_enabled_is_a_decoder_without_the_feature(workdir):
     malloc, free = _libc()
     for s in (BREF, next(s for s in DPB_STREAMS if s[0] == "crop_rect")):
         data = gen(workdir, *s)
-        new, old = port_resized_lib(), port_motion_lib()
+        new, old = port_outputs_lib(), checkers.load("port")
         assert pkg.decode_bytes(data, new, errors=True) == pkg.decode_bytes(data, old, errors=True)
         a, calls_new = with_alloc_cb(new, data, malloc, free)
         b, calls_old = with_alloc_cb(old, data, malloc, free)
@@ -350,7 +296,7 @@ def test_libraries_export_the_resized_api():
 # ---- 6. the device against the restatement ----
 def same_as_restatement(data, fmt, tw, th, n_threads=0, label=""):
     g, gc = pkg.decode_bytes(data, pkg.load(), n_threads, errors=True, resized=(fmt, tw, th))
-    p, pc = pkg.decode_bytes(data, port_resized_lib(), n_threads, errors=True, resized=(fmt, tw, th))
+    p, pc = pkg.decode_bytes(data, port_outputs_lib(), n_threads, errors=True, resized=(fmt, tw, th))
     assert gc == pc and [f[:5] for f in g] == [f[:5] for f in p], label
     for a, b in zip(g, p):
         assert a[-1]["format"] == b[-1]["format"] == fmt and a[-1]["log2_scale"] == b[-1]["log2_scale"] == -1, label
@@ -448,7 +394,7 @@ def test_device_matches_restatement_on_damaged_streams_and_with_threads(workdir)
     for t in (1, 3):
         for fmt, tw, th in ((NV12, 38, 26), (I420, 0, 100)):
             g = pkg.decode_bytes(data, pkg.load(), t, motion=True, resized=(fmt, tw, th))[0]
-            p = pkg.decode_bytes(data, port_resized_lib(), t, motion=True, resized=(fmt, tw, th))[0]
+            p = pkg.decode_bytes(data, port_outputs_lib(), t, motion=True, resized=(fmt, tw, th))[0]
             assert [f[:4] for f in g] == [f[:4] for f in p] and all(same_packed(a[-1], b[-1]) for a, b in zip(g, p))
             assert all(np.array_equal(a[-2][m], b[-2][m]) for a, b in zip(g, p) for m in b[-2])
 
@@ -458,7 +404,7 @@ def _stats(data, resized):
     lib = pkg.load()
     lib.e264b_of_decoder.restype = ctypes.c_void_p; lib.e264b_of_decoder.argtypes = [ctypes.c_void_p]
     lib.e264b_stats.argtypes = [ctypes.c_void_p] + [ctypes.POINTER(ctypes.c_uint64)] * 3
-    dec = new_decoder(lib, resized)
+    dec = new_decoder(lib, resized=resized)
     frames = []
     loop(lib, dec, data, lambda f: frames.append(pkg._frame_bytes(f)))
     s = [ctypes.c_uint64() for _ in range(3)]

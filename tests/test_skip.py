@@ -5,12 +5,13 @@ decoder's own full decode (pinned to the reference decoder elsewhere, and here f
 tests/golden/skip.json): a skip mode outputs the full decode's frames with the skipped pictures removed.
 
 CPU tests run the product's host sources over the plain-C restatement with error maps and the motion export
-(tests/native/port_motion_backend.c, built by tests/test_motion_export.py); the GPU tests compare the device with it."""
+(tests/native/port_outputs_backend.c, built by tests/checkers.py); the GPU tests compare the device with it."""
 import ctypes, errno, functools, hashlib, json, os
 import pytest
 from conftest import ROOT, STREAMS, DPB_STREAMS, make_stream, md5_frames, have
-from test_mb_errors import _nals, _slice_head, _damaged
-from test_motion_export import port_motion_lib
+from test_mb_errors import _nals, _slice_head
+from api_helpers import lib_of, _damaged
+from checkers import port_outputs_lib
 import edge264_b200 as pkg
 import checkers
 
@@ -48,10 +49,6 @@ def pictures(data):
 
 def kept(p, mode):
     return mode == NONE or (mode == NONREF and p["ref"] > 0) or (mode == NONKEY and (p["type"] == 5 or p["slices"][0] == 2))
-
-
-def lib_of(backend):
-    return pkg.load() if backend == "gpu" else port_motion_lib()
 
 
 def decode(data, backend="port", n_threads=0, skip=NONE, motion=False, before=None, after=None):
@@ -288,7 +285,7 @@ def test_skipped_slice_data_is_not_parsed(workdir):
 
 
 def test_damaged_streams_keep_the_record_contract(workdir, monkeypatch):
-    lib = port_motion_lib()
+    lib = port_outputs_lib()
     monkeypatch.setenv("E264_CHECK_RECORDS", "1")
     for name, seed, data in _damaged(workdir):
         for mode in (NONREF, NONKEY):
@@ -299,7 +296,7 @@ def test_damaged_streams_keep_the_record_contract(workdir, monkeypatch):
 
 # ---- 6. API ----
 def test_api_errors():
-    lib = port_motion_lib()
+    lib = port_outputs_lib()
     assert lib.edge264_set_skip(None, NONREF) == errno.EINVAL
     dec = lib.edge264_alloc(0, None, None, 0, None, None, None)
     for mode in (3, -1, 100):
