@@ -895,6 +895,86 @@ extern "C" int e264b_kat_batch(int fn, const uint8_t *modes, const uint8_t *bord
 	return 0;
 }
 
+/* ---- batched residual entry point (tests/test_residual_spec.py -m gpu): the kernels' own residual_stage over n
+ * records in one launch, a warp per record.  Each record's coefficient run is staged 16-byte aligned in shared memory, as
+ * the kernels stage it by cp.async.bulk; the slice records stay in global memory, where idct4x4 reads the scaling lists
+ * with __ldg.  out + 384 i receives ws->res of record i: the luma residual y*16+x, then Cb and Cr 8x8. */
+template <bool LUMA>
+__global__ void e264_kat_residual_kernel(const E264MbRec *recs, const E264SliceRec *slices, const int16_t *pool, int16_t *out) {
+	__shared__ WarpSmem wsm;
+	__shared__ __align__(16) int16_t coef[RES_COEF_MAX];
+	WarpSmem *ws = &wsm;
+	const int lane = threadIdx.x;
+	const E264MbRec *g = recs + blockIdx.x;
+	if (lane < 12) ws->rec4[lane] = ((const uint4 *)g)[lane];
+	const uint4 *run = (const uint4 *)(pool + g->coef_off);   /* the pool carries RES_COEF_MAX levels of padding */
+	for (int i = lane; i < RES_COEF_MAX / 8; i += 32) ((uint4 *)coef)[i] = run[i];
+	__syncwarp();
+	const E264MbRec *r = (const E264MbRec *)ws->rec4;
+	residual_stage<LUMA>(ws, r, slices + r->slice_idx, coef, lane);
+	uint4 *o = (uint4 *)(out + (size_t)blockIdx.x * 384);
+	for (int i = lane; i < 48; i += 32) o[i] = ((const uint4 *)ws->res)[i];
+}
+extern "C" int e264b_kat_residual(const E264MbRec *recs, int n, const E264SliceRec *slices, int n_slices, const int16_t *pool, int n_coefs, int luma_only, int16_t *out) {
+	if (n <= 0 || n_slices <= 0 || n_coefs < 0 || n_coefs % 8) return -1;
+	for (int i = 0; i < n; i++)
+		if (recs[i].slice_idx >= n_slices || recs[i].coef_off % 8 || recs[i].coef_off > (uint32_t)n_coefs) return -1;
+	/* every part starts on 16 bytes: the pool and the output are copied as uint4 (a slice record is 1128 = 8 mod 16 bytes) */
+	const auto up16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+	const size_t rb = up16((size_t)n * sizeof(E264MbRec)), sb = up16((size_t)n_slices * sizeof(E264SliceRec)), pb = up16(((size_t)n_coefs + RES_COEF_MAX) * 2);
+	uint8_t *d = NULL;
+	CK(cudaMalloc(&d, rb + sb + pb + (size_t)n * 768));
+	E264MbRec *d_recs = (E264MbRec *)d;
+	E264SliceRec *d_slices = (E264SliceRec *)(d + rb);
+	int16_t *d_pool = (int16_t *)(d + rb + sb), *d_out = (int16_t *)(d + rb + sb + pb);
+	CK(cudaMemcpy(d_recs, recs, (size_t)n * sizeof(E264MbRec), cudaMemcpyHostToDevice));
+	CK(cudaMemcpy(d_slices, slices, (size_t)n_slices * sizeof(E264SliceRec), cudaMemcpyHostToDevice));
+	CK(cudaMemset(d_pool, 0, pb)); CK(cudaMemcpy(d_pool, pool, (size_t)n_coefs * 2, cudaMemcpyHostToDevice));
+	if (luma_only) e264_kat_residual_kernel<true><<<n, 32>>>(d_recs, d_slices, d_pool, d_out);
+	else e264_kat_residual_kernel<false><<<n, 32>>>(d_recs, d_slices, d_pool, d_out);
+	CK(cudaGetLastError()); CK(cudaDeviceSynchronize());
+	CK(cudaMemcpy(out, d_out, (size_t)n * 768, cudaMemcpyDeviceToHost));
+	cudaFree(d);
+	return 0;
+}
+
+/* ---- batched interpolation entry point (tests/test_pixel_spec.py -m gpu): the inter kernel's window loads and
+ * interpolation over n draws in one launch, a thread per draw.  The plane (`bytes` bytes, rows `stride` apart, w x h
+ * samples) is copied to the start of a device allocation, as a frame slot's luma plane starts one.  Draw i is
+ * draws[4i .. 4i+3] = (x, y, xFrac, yFrac): the integer position of the block's top-left sample, anywhere in or outside
+ * the plane.  Luma: mc_load_luma + mc_luma4x4, quarter-sample fractions, 16 bytes of out per draw (4x4, raster).
+ * Chroma: mc_load_chroma + mc_chroma2x2, eighth-sample fractions, 4 bytes per draw (2x2, raster). */
+__global__ void e264_kat_inter_kernel(int chroma, const uint8_t *plane, int stride, int w, int h, const int32_t *draws, int n, uint8_t *out) {
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const int x = draws[4 * i], y = draws[4 * i + 1], fx = draws[4 * i + 2], fy = draws[4 * i + 3];
+	if (chroma) {
+		uint32_t c[3];
+		mc_load_chroma(plane, stride, w, h, x, y, c);
+		((uint32_t *)out)[i] = mc_chroma2x2(c[0], c[1], c[2], fx, fy);
+	} else {
+		uint32_t win[9][3], o[4];
+		mc_load_luma(plane, stride, w, h, x - 2, y - 2, win);
+		mc_luma4x4(win, fx, fy, o);
+		((uint4 *)out)[i] = make_uint4(o[0], o[1], o[2], o[3]);
+	}
+}
+extern "C" int e264b_kat_inter(int chroma, const uint8_t *plane, int stride, int w, int h, int bytes, const int32_t *draws, int n, uint8_t *out) {
+	if (n <= 0 || w <= 0 || h <= 0 || stride < w || stride % 4 || bytes < (h - 1) * stride + w) return -1;
+	const size_t ob = (size_t)n * (chroma ? 4 : 16), pb = ((size_t)bytes + 64 + 15) & ~(size_t)15;   /* the aligned row loads read up to 3 bytes past a row */
+	uint8_t *d = NULL;
+	CK(cudaMalloc(&d, pb + (size_t)n * 16 + ob));
+	uint8_t *d_plane = d, *d_out = d + pb + (size_t)n * 16;
+	int32_t *d_draws = (int32_t *)(d + pb);
+	CK(cudaMemset(d_plane, 0, pb)); CK(cudaMemcpy(d_plane, plane, bytes, cudaMemcpyHostToDevice));
+	CK(cudaMemcpy(d_draws, draws, (size_t)n * 16, cudaMemcpyHostToDevice));
+	e264_kat_inter_kernel<<<(n + 127) / 128, 128>>>(chroma, d_plane, stride, w, h, d_draws, n, d_out);
+	CK(cudaGetLastError()); CK(cudaDeviceSynchronize());
+	CK(cudaMemcpy(out, d_out, ob, cudaMemcpyDeviceToHost));
+	cudaFree(d);
+	return 0;
+}
+
 /* ---- backend vtable for decoder.c ---- */
 static int be_create(void **ctx) { return e264b_create((E264bDevice **)ctx); }
 static void be_destroy(void *ctx) { e264b_destroy((E264bDevice *)ctx); }

@@ -81,6 +81,12 @@ int      e264b_replay_frames(E264bDevice *dev, uint8_t *out);  /* every kept pic
 int      e264b_kat(int fn, int mode, const uint8_t *in, int in_bytes, uint8_t *out, int w, int h);
 /* the intra predictors (fn 0-3) over n draws in one launch: modes[n], borders 66 bytes and out 256 bytes per draw (recon.cu) */
 int      e264b_kat_batch(int fn, const uint8_t *modes, const uint8_t *borders, int n, uint8_t *out);
+/* the kernels' residual_stage over n records (a warp each, luma-only instantiation when luma_only): levels at
+ * pool[recs[i].coef_off], slices[recs[i].slice_idx]; out receives 384 int16 per record, Y 16x16 then Cb, Cr 8x8 (recon.cu) */
+int      e264b_kat_residual(const struct E264MbRec *recs, int n, const struct E264SliceRec *slices, int n_slices, const int16_t *pool, int n_coefs, int luma_only, int16_t *out);
+/* the inter kernel's window loads and interpolation over n draws (x, y, xFrac, yFrac) of a w x h plane: a 4x4 luma block
+ * (16 bytes of out each) or, with chroma set, a 2x2 chroma block (4 bytes each) (recon.cu) */
+int      e264b_kat_inter(int chroma, const uint8_t *plane, int stride, int w, int h, int bytes, const int32_t *draws, int n, uint8_t *out);
 E264bDevice *e264b_of_decoder(struct Edge264Decoder *dec);
 
 #ifdef __cplusplus

@@ -1,5 +1,6 @@
 """The pixel equations of ITU-T H.264 (04/2017) for 8-bit 4:2:0, written in numpy from the standard's text: intra prediction
-(8.3.1.2, 8.3.2.2, 8.3.3, 8.3.4), chroma sample interpolation (8.4.2.2.2) and weighted sample prediction (8.4.2.3).
+(8.3.1.2, 8.3.2.2, 8.3.3, 8.3.4), luma and chroma sample interpolation (8.4.2.2.1, 8.4.2.2.2) and weighted sample
+prediction (8.4.2.3).
 
 Every function works on n draws at once, in int64.  An intra neighbourhood is three arrays: `corner` (n,) = p[-1,-1],
 `top` (n, 16) = p[0..15,-1] (Intra4x4 reads 8 of them, chroma 8), `left` (n, 16) = p[-1,0..15].  `un` holds the
@@ -7,8 +8,8 @@ unavailable neighbours as the records carry them: A (left) = 1, B (top) = 2, C (
 is only defined where the neighbours it requires are available (REQUIRES); samples of unavailable neighbours are never
 read, whatever they hold.
 
-The one deviation of the reference decoder that the project reproduces is stated apart, as a named function with its
-citation (ref_wp_bi_int16); the standard's formulas do not contain it."""
+The deviations of the reference decoder that the project reproduces are stated apart, as named functions with their
+citations (ref_wp_bi_int16, ref_luma_j_int16); the standard's formulas do not contain them."""
 import numpy as np
 
 A, B, C, D = 1, 2, 4, 8
@@ -250,3 +251,77 @@ def ref_wp_bi_int16(p0, p1, w0, w1, o0, o1, logWD):
     clips to 255; at logWD <= 6 the saturated value still clips to the same 0 or 255)."""
     logWD = np.asarray(logWD, np.int64)
     return np.clip(np.clip(bi_sum(p0, p1, w0, w1, o0, o1, logWD), -32768, 32767) >> (logWD + 1), 0, 255)
+
+
+# ---- luma sample interpolation ----
+def _tap6(a, b, c, d, e, f):
+    return a - 5 * b + 20 * c + 20 * d - 5 * e + f
+
+
+# Table 8-12: the sample each (xFrac, yFrac) takes
+LUMA_SAMPLE = {(0, 0): "G", (0, 1): "d", (0, 2): "h", (0, 3): "n", (1, 0): "a", (1, 1): "e", (1, 2): "i", (1, 3): "p",
+               (2, 0): "b", (2, 1): "f", (2, 2): "j", (2, 3): "q", (3, 0): "c", (3, 1): "g", (3, 2): "k", (3, 3): "r"}
+J_FRACTIONS = [(2, 1), (1, 2), (2, 2), (3, 2), (2, 3)]   # f, i, j, k, q: the samples that take j
+
+
+def _luma_gather(plane, xInt, yInt):
+    """P(dx, dy): the full sample at (xInt + dx, yInt + dy) of each draw in the (H, W) plane, the position clamped into
+    the picture (8-228, 8-229)."""
+    plane = np.asarray(plane)
+    xInt, yInt = _i64(xInt, yInt)
+    h, w = plane.shape
+    return lambda dx, dy: plane[np.clip(yInt + dy, 0, h - 1), np.clip(xInt + dx, 0, w - 1)].astype(np.int64)
+
+
+def _luma_samples(P, jval):
+    """8-243..8-261: every sample of Table 8-12 by name, from the full samples P and the centre sample j"""
+    clip = lambda v: np.clip(v, 0, 255)
+    b1, h1 = _tap6(*[P(dx, 0) for dx in range(-2, 4)]), _tap6(*[P(0, dy) for dy in range(-2, 4)])      # 8-241, 8-242
+    s1, m1 = _tap6(*[P(dx, 1) for dx in range(-2, 4)]), _tap6(*[P(1, dy) for dy in range(-2, 4)])
+    b, h, s, m = (clip((v + 16) >> 5) for v in (b1, h1, s1, m1))                                    # 8-243, 8-244, 8-247, 8-248
+    G, H, M, j = P(0, 0), P(1, 0), P(0, 1), jval
+    avg = lambda u, v: (u + v + 1) >> 1
+    return {"G": G, "b": b, "h": h, "j": j, "a": avg(G, b), "c": avg(H, b), "d": avg(G, h), "n": avg(M, h),      # 8-250..8-257
+            "f": avg(b, j), "i": avg(h, j), "k": avg(j, m), "q": avg(j, s),
+            "e": avg(b, h), "g": avg(b, m), "p": avg(h, s), "r": avg(m, s)}                           # 8-258..8-261
+
+
+def luma_j1(P):
+    """8-245: j1 = cc - 5 dd + 20 h1 + 20 m1 - 5 ee + ff, from the vertical intermediates of columns -2..3"""
+    return _tap6(*[_tap6(*[P(dx, dy) for dy in range(-2, 4)]) for dx in range(-2, 4)])
+
+
+def luma_sample(plane, xInt, yInt, xFrac, yFrac):
+    """8.4.2.2.1: one luma sample per draw at integer position (xInt, yInt) and quarter-sample fraction (xFrac, yFrac);
+    positions outside the plane are clamped."""
+    P = _luma_gather(plane, xInt, yInt)
+    smp = _luma_samples(P, np.clip((luma_j1(P) + 512) >> 10, 0, 255))                             # 8-246
+    xFrac, yFrac = _i64(xFrac, yFrac)
+    return np.select([(xFrac == fx) & (yFrac == fy) for fx, fy in LUMA_SAMPLE], [smp[v] for v in LUMA_SAMPLE.values()])
+
+
+def luma_j_int16(P, hfirst):
+    """ref_luma_j_int16's centre sample from the full samples P, and its inner sum t unwrapped"""
+    s6 = ([_tap6(*[P(dx, dy) for dx in range(-2, 4)]) for dy in range(-2, 4)] if hfirst else      # b1 of rows -2..3
+          [_tap6(*[P(dx, dy) for dy in range(-2, 4)]) for dx in range(-2, 4)])                     # h1 of columns -2..3
+    af, be, cd = s6[0] + s6[5], s6[1] + s6[4], s6[2] + s6[3]
+    t = ((af - be) >> 2) + (cd - be)
+    t16 = ((t + 32768) & 65535) - 32768
+    return np.clip(((t16 >> 2) + cd + 32) >> 6, 0, 255), t
+
+
+def luma_j_inner(plane, xInt, yInt, xFrac):
+    """the inner sum t of ref_luma_j_int16, unwrapped, in the pass order xFrac selects"""
+    P = _luma_gather(plane, xInt, yInt)
+    return np.where(np.asarray(xFrac) == 2, luma_j_int16(P, True)[1], luma_j_int16(P, False)[1])
+
+
+def ref_luma_j_int16(plane, xInt, yInt, xFrac, yFrac):
+    """DEVIATION of the reference decoder (edge264_inter.c:4-9, :559-640), reproduced by the restatement and the device:
+    j is ((t >> 2) + (c+d) + 32) >> 6 with t = ((a+f - (b+e)) >> 2) + (c+d - (b+e)) WRAPPED to int16, a..f the six
+    first-pass sums, horizontal first for xFrac 2 (f, j, q) and vertical first for odd xFrac (i, k).  Without the wrap
+    this is (j1 + 512) >> 10 exactly (nested floors of integer sums); with it, it differs where t leaves int16."""
+    P = _luma_gather(plane, xInt, yInt)
+    xFrac, yFrac = _i64(xFrac, yFrac)
+    smp = _luma_samples(P, np.where(xFrac == 2, luma_j_int16(P, True)[0], luma_j_int16(P, False)[0]))
+    return np.select([(xFrac == fx) & (yFrac == fy) for fx, fy in LUMA_SAMPLE], [smp[v] for v in LUMA_SAMPLE.values()])

@@ -330,3 +330,233 @@ def test_explicit_bi_prediction_matches_the_standard_except_at_logwd_7(mcl):
 
 
 EXT_DIFFERING = 326142   # samples of the bound sweep where the reference's saturation changes the result
+
+
+# ---- luma interpolation ----
+def luma_planes():
+    """Small planes: random, 0/255 random, and 0/255 period-3 patterns (a row pattern XOR a column pattern, both of
+    period 3, every phase), of sizes down to 4x4."""
+    rng = np.random.default_rng(17)
+    out = []
+    for k, (h, w) in enumerate(((16, 16), (7, 11), (13, 5), (4, 4), (9, 20), (12, 8))):
+        out.append(rng.integers(0, 256, (h, w)))
+        out.append(255 * rng.integers(0, 2, (h, w)))
+        for px in range(3):
+            a, b = rng.integers(0, 2, 3), rng.integers(0, 2, 3)
+            out.append(255 * (a[(np.arange(w) + px) % 3][None, :] ^ b[(np.arange(h) + k) % 3][:, None]))
+    return out
+
+
+def luma_draws(plane, rng, n):
+    """n (x, y, xFrac, yFrac) with positions up to 8 samples outside the plane, every fraction equally often"""
+    h, w = plane.shape
+    f = np.arange(n) % 16
+    return rng.integers(-8, w + 8, n), rng.integers(-8, h + 8, n), f & 3, f >> 2
+
+
+def check_luma(name, got, plane, x, y, fx, fy):
+    """got equals ref_luma_j_int16 everywhere and 8.4.2.2.1 wherever the inner sum of j stays in int16 or the fraction
+    does not take j; returns the number of samples that differ from the standard"""
+    std, dev = spec.luma_sample(plane, x, y, fx, fy), spec.ref_luma_j_int16(plane, x, y, fx, fy)
+    bad = np.nonzero(got != dev)[0]
+    assert len(bad) == 0, f"{name}: {len(bad)} samples differ from the reference's arithmetic, first at ({x[bad[0]]}, {y[bad[0]]}) frac ({fx[bad[0]]}, {fy[bad[0]]}): want {dev[bad[0]]} got {got[bad[0]]}"
+    t = spec.luma_j_inner(plane, x, y, fx)
+    takes_j = np.isin(fx + 4 * fy, [a + 4 * b for a, b in spec.J_FRACTIONS])
+    diff = got != std
+    assert not (diff & ~(takes_j & ((t < -32768) | (t > 32767)))).any(), f"{name}: differs from 8.4.2.2.1 where j's inner sum stays in int16"
+    return int(diff.sum())
+
+
+def blocks_to_samples(plane, x, y, fx, fy):
+    """the 16 sample draws of 4x4 blocks at (x, y): (plane, x, y, fx, fy) repeated per sample, raster in the block"""
+    dy, dx = np.divmod(np.arange(16), 4)
+    rep = lambda a: np.repeat(np.asarray(a), 16)
+    return rep(x) + np.tile(dx, len(x)), rep(y) + np.tile(dy, len(x)), rep(fx), rep(fy)
+
+
+def windows(plane, x, y):
+    """the 9x9 windows at (x - 2, y - 2) the device loads, positions clamped into the plane, as nine rows of three words"""
+    h, w = plane.shape
+    r, k = np.arange(9), np.arange(12)
+    win = plane[np.clip(np.asarray(y)[:, None, None] - 2 + r[None, :, None], 0, h - 1), np.clip(np.asarray(x)[:, None, None] - 2 + k[None, None, :], 0, w - 1)]
+    win[:, :, 9:] = 0
+    return rows_to_words(win)
+
+
+def rows_to_words(win):
+    b = np.asarray(win, np.uint32).reshape(len(win), 9, 3, 4)
+    return np.ascontiguousarray(b[..., 0] | b[..., 1] << 8 | b[..., 2] << 16 | b[..., 3] << 24)
+
+
+def mcl_luma(mcl, words, fx, fy):
+    n = len(words)
+    f, g = i32(fx, fy)
+    out = np.zeros((n, 4), np.uint32)
+    mcl.mcl_luma4x4(n, ptr(words), ptr(f), ptr(g), ptr(out))
+    return unpack(out.ravel())      # (n * 16,): the blocks' samples, raster
+
+
+def test_luma_interpolation_matches_the_standard(mcl):
+    """8.4.2.2.1 on the restatement (port_mc_luma_sample, per sample, with its clamping) and on mc_luma4x4 (4x4 blocks of
+    the host build, windows clamped as mc_load_luma clamps them): every fraction, random, 0/255 and period-3 planes,
+    positions up to 8 samples outside them.  The only differences from the standard are at f, i, j, k and q, where the
+    inner sum of j leaves int16, and they equal ref_luma_j_int16."""
+    lib = ctypes.CDLL(_LIBS["port"])
+
+    class Plane(ctypes.Structure):
+        _fields_ = [("p", ctypes.c_void_p), ("stride", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
+    lib.port_mc_luma_sample.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+    rng = np.random.default_rng(19)
+    n_port = n_mc = d_port = d_mc = 0
+    for plane in luma_planes():
+        p8 = np.ascontiguousarray(plane, np.uint8)
+        pl = Plane(p8.ctypes.data, p8.shape[1], p8.shape[1], p8.shape[0])
+        x, y, fx, fy = luma_draws(plane, rng, 640)
+        got = np.array([lib.port_mc_luma_sample(ctypes.byref(pl), int(a), int(b), int(c), int(d)) for a, b, c, d in zip(x, y, fx, fy)])
+        d_port += check_luma("port_mc_luma_sample", got, plane, x, y, fx, fy)
+        n_port += len(x)
+        x, y, fx, fy = luma_draws(plane, rng, 640)
+        got = mcl_luma(mcl, windows(plane, x, y), fx, fy)
+        d_mc += check_luma("mc_luma4x4", got, plane, *blocks_to_samples(plane, x, y, fx, fy))
+        n_mc += 16 * len(x)
+    print(f"luma interpolation: {n_port} restatement samples ({d_port} differ from the standard), {n_mc} mc_luma4x4 samples ({d_mc})")
+
+
+def xor_sweep():
+    """Every 9x9 window 255 (X[x] ^ Y[y]) of two 9-bit patterns X, Y: 262 144 windows"""
+    bits = (np.arange(512)[:, None] >> np.arange(9)) & 1
+    return (255 * (bits[None, :, None, :] ^ bits[:, None, :, None])).reshape(-1, 9, 9).astype(np.uint8)
+
+
+def test_luma_extreme_sweep_differs_only_at_j(mcl):
+    """mc_luma4x4 over the XOR sweep at all 16 fractions (67 M samples) against the standard: the differing samples all
+    take j, all have j's inner sum outside int16, and equal ref_luma_j_int16; their number is pinned."""
+    win = xor_sweep()
+    words = rows_to_words(np.concatenate([win, np.zeros((len(win), 9, 3), np.uint8)], 2))
+    n, total = len(win), 0
+    per_frac = {}
+    for fy in range(4):
+        for fx in range(4):
+            got = mcl_luma(mcl, words, np.full(n, fx), np.full(n, fy)).reshape(n, 4, 4)
+            diff = 0
+            for by in range(4):
+                for bx in range(4):
+                    P = lambda dx, dy: win[:, 2 + by + dy, 2 + bx + dx].astype(np.int64)
+                    std = spec._luma_samples(P, np.clip((spec.luma_j1(P) + 512) >> 10, 0, 255))[spec.LUMA_SAMPLE[fx, fy]]
+                    jd, t = spec.luma_j_int16(P, fx == 2)
+                    dev = spec._luma_samples(P, jd)[spec.LUMA_SAMPLE[fx, fy]]
+                    g = got[:, by, bx]
+                    assert np.array_equal(g, dev), f"mc_luma4x4 frac ({fx}, {fy}) sample ({bx}, {by}): not the reference's arithmetic"
+                    d = g != std
+                    if (fx, fy) not in spec.J_FRACTIONS:
+                        assert not d.any(), f"frac ({fx}, {fy}) differs from the standard"
+                    assert not (d & (t >= -32768) & (t <= 32767)).any()
+                    diff += int(d.sum())
+            per_frac[spec.LUMA_SAMPLE[fx, fy]] = diff
+            total += 16 * n
+    ndiff = sum(per_frac.values())
+    print(f"luma sweep: {total} samples, {ndiff} differ from the standard:", {k: v for k, v in per_frac.items() if v})
+    assert ndiff == SWEEP_DIFFERING > 0, ndiff
+
+
+SWEEP_DIFFERING = 20480   # samples of the XOR sweep where the reference's int16 centre sum changes the result
+
+
+def order_plane():
+    """The windows on which the order of j's two passes shows: each window of the XOR sweep whose j at sample (2, 2)
+    leaves int16 in either order, with one sample of its 6x6 footprint set to 0, 128 or 255, kept where the wrapped j
+    of the horizontal-first and of the vertical-first order differ.  They are laid side by side in one 9-row plane,
+    window i in columns 9 i .. 9 i + 8, so the block at (9 i + 2, 2) reads window i alone."""
+    win = xor_sweep().astype(np.int64)
+    P = lambda dx, dy: win[:, 2 + dy, 2 + dx]
+    th, tv = spec.luma_j_int16(P, True)[1], spec.luma_j_int16(P, False)[1]
+    wraps = (th < -32768) | (th > 32767) | (tv < -32768) | (tv > 32767)
+    base = win[wraps]
+    out = []
+    for pos in range(36):
+        for v in (0, 128, 255):
+            w = base.copy()
+            w[:, pos // 6, pos % 6] = v
+            out.append(w)
+    w = np.concatenate(out)
+    P = lambda dx, dy: w[:, 2 + dy, 2 + dx]
+    w = w[spec.luma_j_int16(P, True)[0] != spec.luma_j_int16(P, False)[0]]
+    return np.ascontiguousarray(w.transpose(1, 0, 2).reshape(9, -1)), len(w)
+
+
+def order_draws(n):
+    """every j-taking fraction at the block of each window of order_plane"""
+    f = np.array(spec.J_FRACTIONS)
+    x = np.tile(9 * np.arange(n) + 2, len(f))
+    return x, np.full(len(x), 2), np.repeat(f[:, 0], n), np.repeat(f[:, 1], n)
+
+
+def test_luma_pass_order_of_j(mcl):
+    """The restatement and mc_luma4x4 on the windows where the order of j's passes changes the result (order_plane):
+    horizontal first for f, j, q and vertical first for i, k, as ref_luma_j_int16; the samples that differ from the
+    standard are pinned."""
+    lib = ctypes.CDLL(_LIBS["port"])
+
+    class Plane(ctypes.Structure):
+        _fields_ = [("p", ctypes.c_void_p), ("stride", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int)]
+    lib.port_mc_luma_sample.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+    plane, n = order_plane()
+    assert n == ORDER_WINDOWS, n
+    x, y, fx, fy = order_draws(n)
+    p8 = np.ascontiguousarray(plane, np.uint8)
+    pl = Plane(p8.ctypes.data, p8.shape[1], p8.shape[1], p8.shape[0])
+    got = np.array([lib.port_mc_luma_sample(ctypes.byref(pl), int(a), int(b), int(c), int(d)) for a, b, c, d in zip(x, y, fx, fy)])
+    d_port = check_luma("port_mc_luma_sample", got, plane, x, y, fx, fy)
+    got = mcl_luma(mcl, windows(plane, x, y), fx, fy)
+    d_mc = check_luma("mc_luma4x4", got, plane, *blocks_to_samples(plane, x, y, fx, fy))
+    print(f"pass order of j: {n} windows x {len(spec.J_FRACTIONS)} fractions, {d_port} restatement samples and {d_mc} "
+          f"mc_luma4x4 samples differ from the standard")
+    assert (d_port, d_mc) == ORDER_DIFFERING and d_port > 0, (d_port, d_mc)
+
+
+ORDER_WINDOWS = 4096     # windows of order_plane
+ORDER_DIFFERING = (10240, 14360)   # restatement samples and mc_luma4x4 samples (whole blocks) of test_luma_pass_order_of_j
+                                   # that differ from the standard
+
+
+def kat_inter(lib, chroma, plane, x, y, fx, fy):
+    """e264b_kat_inter over draws of one plane, laid out with the stride of a frame slot (the width; a multiple of 4)"""
+    h, w = plane.shape
+    stride = (w + 3) & ~3
+    buf = np.zeros((h, stride), np.uint8)
+    buf[:, :w] = plane
+    buf[:, w:] = 77      # samples past the width must never be read as the plane's
+    draws = np.ascontiguousarray(np.stack([x, y, fx, fy], 1), np.int32)
+    out = np.zeros((len(x), 4 if chroma else 16), np.uint8)
+    assert lib.e264b_kat_inter(int(chroma), buf.ctypes.data, stride, w, h, buf.size, draws.ctypes.data, len(x), out.ctypes.data) == 0
+    return out.astype(np.int64)
+
+
+@pytest.mark.gpu
+def test_device_interpolation_matches_the_standard():
+    """The inter kernel's mc_load_luma + mc_luma4x4 and mc_load_chroma + mc_chroma2x2 through e264b_kat_inter, with the
+    device's own clamping at the plane's edges: the planes and positions of the CPU test, every fraction, and the windows
+    on which the order of j's passes shows."""
+    lib = ctypes.CDLL(_LIBS["gpu"])
+    lib.e264b_kat_inter.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+    rng = np.random.default_rng(23)
+    n_l = n_c = d_l = 0
+    for plane in luma_planes():
+        x, y, fx, fy = luma_draws(plane, rng, 4096)
+        got = kat_inter(lib, False, plane, x, y, fx, fy).ravel()
+        d_l += check_luma("device luma", got, plane, *blocks_to_samples(plane, x, y, fx, fy))
+        n_l += got.size
+        h, w = plane.shape
+        x, y = rng.integers(-8, w + 8, 4096), rng.integers(-8, h + 8, 4096)
+        f = np.arange(4096) % 64
+        got = kat_inter(lib, True, plane, x, y, f & 7, f >> 3)
+        want = np.stack([spec.chroma_sample(plane, x + dx, y + dy, f & 7, f >> 3) for dy in (0, 1) for dx in (0, 1)], 1)
+        bad = np.nonzero((got != want).any(1))[0]
+        assert len(bad) == 0, f"device chroma: {len(bad)} blocks differ, first at ({x[bad[0]]}, {y[bad[0]]}) frac {f[bad[0]]}: want {want[bad[0]]} got {got[bad[0]]}"
+        n_c += got.size
+    plane, n = order_plane()
+    x, y, fx, fy = order_draws(n)
+    got = kat_inter(lib, False, plane, x, y, fx, fy).ravel()
+    d_l += check_luma("device luma, pass order of j", got, plane, *blocks_to_samples(plane, x, y, fx, fy))
+    n_l += got.size
+    print(f"device interpolation: {n_l} luma samples ({d_l} differ from the standard, all at j), {n_c} chroma samples")
