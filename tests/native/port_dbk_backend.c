@@ -1,6 +1,8 @@
 /* port_dbk_backend.c — TEST INFRASTRUCTURE ONLY.  The CPU restatement's backend (oracle/port_backend.c) with every picture
  * written out for the deblocking test (tests/test_deblock_spec.py): when E264_DBK_DUMP names a file, each submit appends
- * the picture's E264PicDesc, records and slice records, then the picture before deblocking, then the picture itself.  The
+ * the picture's E264PicDesc, records, slice records and levels, then the picture before deblocking, then the picture itself
+ * (tests/picture_dumps.py reads the file).  Each configure and each fill_slot (the frames of a frame_num gap, decoder.c
+ * fill_frame_num_gap, and skipped references, fill_skipped) is written as an entry of its own, so that the file says what every frame slot holds.  The
  * picture before deblocking is the same picture reconstructed from its records with MBF_DEBLOCK / MBF_EDGE_* cleared and
  * any_deblock 0 (a picture the record contract allows); it goes to a buffer of its own, and the picture is then
  * reconstructed as parsed, so the frame slots hold what they hold without the dump.  The test links this file with the
@@ -14,6 +16,23 @@ const E264Backend *__real_e264_default_backend(void);
 static E264Backend dbk_backend;
 static E264Staging staged[64];   /* by handle: what acquire_staging handed out */
 
+enum { DUMP_PICTURE = 1, DUMP_FILL = 2, DUMP_CONFIGURE = 3 };   /* the tag before each entry */
+static FILE *dump_open(void) {
+	const char *path = getenv("E264_DBK_DUMP");
+	return path && *path ? fopen(path, "ab") : NULL;
+}
+static int dbk_configure(void *ctx, const E264PicDesc *g, int n_slots) {
+	const int r = __real_e264_default_backend()->configure(ctx, g, n_slots);
+	FILE *f = r ? NULL : dump_open();
+	if (f) { uint32_t tag = DUMP_CONFIGURE; int32_t n = n_slots; fwrite(&tag, 4, 1, f); fwrite(g, sizeof(*g), 1, f); fwrite(&n, 4, 1, f); fclose(f); }
+	return r;
+}
+static int dbk_fill(void *ctx, int slot, int y, int c) {
+	const int r = __real_e264_default_backend()->fill_slot(ctx, slot, y, c);
+	FILE *f = r ? NULL : dump_open();
+	if (f) { uint32_t tag = DUMP_FILL; int32_t v[3] = {slot, y, c}; fwrite(&tag, 4, 1, f); fwrite(v, 4, 3, f); fclose(f); }
+	return r;
+}
 static int dbk_acquire(void *ctx, int slot, E264Staging *out) {
 	const int r = __real_e264_default_backend()->acquire_staging(ctx, slot, out);
 	if (!r && out->handle >= 0 && out->handle < 64) staged[out->handle] = *out;
@@ -39,7 +58,10 @@ static int dbk_submit(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint6
 	if (!r) r = real->wait(ctx, *ticket);
 	FILE *f = r ? NULL : fopen(path, "ab");
 	if (f) {
+		uint32_t tag = DUMP_PICTURE;
+		fwrite(&tag, 4, 1, f);
 		fwrite(pd, sizeof(*pd), 1, f); fwrite(recs, sizeof(E264MbRec), nmb, f); fwrite(st->slices, sizeof(E264SliceRec), (size_t)pd->n_slices, f);
+		fwrite(st->coefs, 2, (size_t)pd->n_coefs, f);
 		fwrite(pre, 1, (size_t)pd->frame_bytes, f); fwrite(host_out, 1, (size_t)pd->frame_bytes, f);
 		fclose(f);
 	} else if (!r) r = -1;
@@ -49,6 +71,8 @@ static int dbk_submit(void *ctx, const E264PicDesc *pd, uint8_t *host_out, uint6
 const E264Backend *__wrap_e264_default_backend(void) {
 	dbk_backend = *__real_e264_default_backend();
 	dbk_backend.name = "port-dbk";
+	dbk_backend.configure = dbk_configure;
+	dbk_backend.fill_slot = dbk_fill;
 	dbk_backend.acquire_staging = dbk_acquire;
 	dbk_backend.submit = dbk_submit;
 	return &dbk_backend;

@@ -14,8 +14,9 @@
  * counters: inflight_max, contexts, ref_slot_in_flight, dst_slot_read_in_flight, and staging_wrapped (pictures submitted
  * while every staging area of the context was in use, so that e264b_acquire_staging had to wait), after one line of
  * pictures per context.
- * --dump DIR (one picture in flight) writes, for every picture of seed k, to DIR/seed_k.bin: its E264PicDesc, records,
- * slice records, the picture before deblocking and the picture after it (tests/test_deblock_spec.py).  The picture
+ * --dump DIR (one picture in flight) writes seed k to DIR/seed_k.bin (the format of tests/picture_dumps.py): the geometry,
+ * the initial fill of every frame slot, then for every picture its E264PicDesc, records, slice records, levels, the
+ * picture before deblocking and the picture after it (tests/test_deblock_spec.py, tests/test_picture_spec.py).  The picture
  * before deblocking is reconstructed first, from a copy of the records with MBF_DEBLOCK / MBF_EDGE_* cleared and
  * any_deblock 0, by the port (--cpu-only) or by the device; then the picture is reconstructed as drawn, so the frame
  * slots hold what they hold without --dump.  The draws are the same with and without it. */
@@ -427,10 +428,18 @@ static void dump_mb(const E264MbRec *recs, const E264SliceRec *slices, int W, in
 	        s->wp_mode, s->luma_log2_wd, s->chroma_log2_wd, s->scaling4x4[0][0], s->scaling8x8[0][0]);
 }
 
-/* --dump: one picture's description, records, slices, the picture before deblocking and after it */
-static void dump_picture(Ctx *c, const E264PicDesc *pd, const E264MbRec *recs, const E264SliceRec *slices, const uint8_t *post) {
+/* --dump entries (tests/picture_dumps.py): a tag, then the entry */
+enum { DUMP_PICTURE = 1, DUMP_FILL = 2, DUMP_CONFIGURE = 3 };
+static void dump_tag(Ctx *c, uint32_t tag) { fwrite(&tag, 4, 1, c->dump); }
+/* the geometry and the number of frame slots, at the start of each seed's file */
+static void dump_configure(Ctx *c) { int32_t n = c->n_slots; dump_tag(c, DUMP_CONFIGURE); fwrite(&c->g, sizeof(c->g), 1, c->dump); fwrite(&n, 4, 1, c->dump); }
+/* a slot set to y on its luma plane and cc after it */
+static void dump_fill(Ctx *c, int slot, int y, int cc) { int32_t v[3] = {slot, y, cc}; dump_tag(c, DUMP_FILL); fwrite(v, 4, 3, c->dump); }
+/* one picture's description, records, slices, levels, the picture before deblocking and after it */
+static void dump_picture(Ctx *c, const E264PicDesc *pd, const E264MbRec *recs, const E264SliceRec *slices, const int16_t *coefs, const uint8_t *post) {
+	dump_tag(c, DUMP_PICTURE);
 	fwrite(pd, sizeof(*pd), 1, c->dump); fwrite(recs, sizeof(E264MbRec), (size_t)c->nmb, c->dump);
-	fwrite(slices, sizeof(E264SliceRec), (size_t)pd->n_slices, c->dump);
+	fwrite(slices, sizeof(E264SliceRec), (size_t)pd->n_slices, c->dump); fwrite(coefs, 2, (size_t)pd->n_coefs, c->dump);
 	fwrite(c->dump_pre, 1, (size_t)pd->frame_bytes, c->dump); fwrite(post, 1, (size_t)pd->frame_bytes, c->dump);
 }
 
@@ -467,7 +476,7 @@ static int retire(Ctx *c, int cpu_only) {
 	c->q_head = (c->q_head + 1) % c->inflight; c->n_out--;
 	if (cpu_only) return 0;
 	if (D.wait(c->dev, p->ticket)) { fprintf(stderr, "picture %d: wait failed\n", p->pic); return 1; }
-	if (c->dump) dump_picture(c, &p->pd, p->recs, p->slices, p->host_out);   /* before the comparison: a picture that fails it is judged too */
+	if (c->dump) dump_picture(c, &p->pd, p->recs, p->slices, p->coefs, p->host_out);   /* before the comparison: a picture that fails it is judged too */
 	const int W = c->g.width_mbs, H = c->g.height_mbs;
 	for (int pl = 0; pl < 3; pl++) {
 		int w = pl ? W * 8 : W * 16, h = pl ? H * 8 : H * 16, stride = pl ? c->g.stride_c : c->g.stride_y;
@@ -528,7 +537,7 @@ static int run_picture(Ctx *c, int pic, int dst, int pcm_content, int cpu_only) 
 	pthread_mutex_lock(&port_mu);
 	port_recon_picture(c->port_frames, &pd, c->recs, c->coefs, c->slices);
 	pthread_mutex_unlock(&port_mu);
-	if (c->dump && cpu_only) dump_picture(c, &pd, c->recs, c->slices, c->port_frames + (size_t)dst * c->g.frame_bytes);
+	if (c->dump && cpu_only) dump_picture(c, &pd, c->recs, c->slices, c->coefs, c->port_frames + (size_t)dst * c->g.frame_bytes);
 	Pending *p = c->q + (c->q_head + c->n_out) % c->inflight;
 	p->pic = pic; p->dst = dst; p->reads = reads; p->pd = pd;
 	if (++c->n_out > cov[C_INFLIGHT_MAX]) cov[C_INFLIGHT_MAX] = c->n_out;
@@ -587,11 +596,13 @@ static void *run_context(void *arg) {
 			}
 			if (c.dump) c.dump_dev = D.host_alloc(c.dev, c.g.frame_bytes);
 		}
+		if (c.dump) dump_configure(&c);
 		for (int s = 0; s < c.n_slots; s++) {   /* every slot starts identical on both sides */
 			int y = rnd(256), cc = rnd(256);
 			uint8_t *f = c.port_frames + (size_t)s * c.g.frame_bytes;
 			memset(f, y, c.g.plane_y); memset(f + c.g.plane_y, cc, c.g.frame_bytes - c.g.plane_y);
 			if (!cpu_only) D.fill(c.dev, s, y, cc);
+			if (c.dump) dump_fill(&c, s, y, cc);
 		}
 		int bad = 0, first_pic = j->total;
 		for (int s = 0; s < c.n_slots && !bad; s++) bad = run_picture(&c, j->total++, s, s % 3, cpu_only);   /* textured references */

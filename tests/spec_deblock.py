@@ -42,9 +42,11 @@ REC = np.dtype([("kind", "u1"), ("flags", "u1"), ("qp", "u1", 3), ("chroma_mode"
                 ("coded", "<u4"), ("coef_off", "<u4"), ("modes", "u1", 16), ("ref_idx", "i1", (2, 4)), ("ref_pic", "i1", (2, 4)),
                 ("err", "u1"), ("reserved", "u1", 15), ("mv", "<i2", (2, 16, 2))])
 SLICE = np.dtype([("filter_offset_a", "i1"), ("filter_offset_b", "i1"), ("deblock_idc", "u1"), ("slice_type", "u1"), ("wp_mode", "u1"),
-                  ("luma_log2_wd", "u1"), ("chroma_log2_wd", "u1"), ("reserved", "u1"), ("rest", "V1120")])
+                  ("luma_log2_wd", "u1"), ("chroma_log2_wd", "u1"), ("reserved", "u1"), ("wp_w", "<i2", (2, 16, 3)), ("wp_o", "<i2", (2, 16, 3)),
+                  ("implicit_w1", "<i2", (16, 16)), ("scaling4x4", "u1", (6, 16)), ("scaling8x8", "u1", (2, 64))])
 PICDESC = np.dtype([(n, "<i4") for n in ("width_mbs", "height_mbs", "stride_y", "stride_c", "plane_y", "frame_bytes", "dst_slot",
-                                          "n_slices", "n_coefs", "any_deblock", "n_intra", "staging", "err_pic")] + [("taint", "<u4")])
+                                          "n_slices", "n_coefs", "any_deblock", "n_intra", "staging")]
+                   + [("err_pic", "u1"), ("luma_only", "u1"), ("reserved", "u1", 2), ("taint", "<u4")])
 assert REC.itemsize == 192 and SLICE.itemsize == 1128 and PICDESC.itemsize == 56
 
 

@@ -9,14 +9,14 @@ standard and read one copy of the tables, so an error they share passes every te
     byte, on the parser's records of the stream sets (CPU backend tests/native/port_dbk_backend.c), on the record
     fuzzer's pictures through the restatement (CPU) and through the device (GPU, independent of the restatement).
 The whole-picture runs print the statement's coverage counts and assert that each is non-zero."""
-import collections, ctypes, glob, os, re, subprocess, tempfile, time
+import collections, ctypes, os, re, subprocess, time
 import numpy as np
 import pytest
-from conftest import ROOT, STREAMS, DPB_STREAMS, make_stream
+from conftest import ROOT, STREAMS, DPB_STREAMS
 from checkers import _LIBS
 from test_limits import LIMITS
-import edge264_b200 as pkg
 import spec_deblock as spec
+from picture_dumps import FUZZ_SEEDS, GEOM, build_fuzzer, load_dump, run_fuzzer, stream_pictures
 
 NATIVE = os.path.join(ROOT, "tests", "native")
 CSRC = os.path.join(ROOT, "edge264_b200", "csrc")
@@ -255,24 +255,6 @@ def test_boundary_strength_matches_the_standard(dbl, port):
 
 
 # ---- whole pictures ----
-def load_dump(path):
-    """The pictures a dump file holds: (PicDesc, records, slices, picture before deblocking, picture after)."""
-    raw = np.fromfile(path, np.uint8)
-    off, pics = 0, []
-    while off < len(raw):
-        pd = raw[off:off + spec.PICDESC.itemsize].view(spec.PICDESC)[0]
-        off += spec.PICDESC.itemsize
-        nmb, ns, fb = int(pd["width_mbs"]) * int(pd["height_mbs"]), int(pd["n_slices"]), int(pd["frame_bytes"])
-        recs = raw[off:off + nmb * spec.REC.itemsize].view(spec.REC)
-        off += nmb * spec.REC.itemsize
-        sl = raw[off:off + ns * spec.SLICE.itemsize].view(spec.SLICE)
-        off += ns * spec.SLICE.itemsize
-        pics.append((pd, recs, sl, raw[off:off + fb], raw[off + fb:off + 2 * fb]))
-        off += 2 * fb
-    return pics
-
-
-GEOM = ("width_mbs", "height_mbs", "stride_y", "stride_c", "plane_y", "frame_bytes")
 
 
 def check_pictures(pics, what):
@@ -323,32 +305,6 @@ def required(cov):
     return {k: cov[k] for k in keys}
 
 
-_built = {}
-
-
-def port_dbk_lib():
-    """The whole edge264 API on the CPU restatement, every picture written out before and after deblocking."""
-    if "lib" not in _built:
-        path = os.path.join(tempfile.mkdtemp(prefix="e264dbk"), "libport_dbk.so")
-        src = [os.path.join(NATIVE, "port_dbk_backend.c"), os.path.join(ROOT, "oracle", "port_backend.c"), os.path.join(ROOT, "oracle", "port_recon.c"),
-               os.path.join(ROOT, "oracle", "record_check.c"), os.path.join(CSRC, "decoder.c"), os.path.join(CSRC, "slice_dec.c")]
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-w", "-o", path] + src + ["-pthread", "-Wl,--wrap=e264_default_backend"], check=True)
-        _built["lib"] = pkg.bind(path)
-    return _built["lib"]
-
-
-def stream_pictures(workdir, tmp_path, name, w, h, args):
-    data = open(make_stream(workdir, name, w, h, args), "rb").read()
-    dump = str(tmp_path / (name + ".dbk"))
-    os.environ["E264_DBK_DUMP"] = dump
-    try:
-        frames, _ = pkg.decode_bytes(data, port_dbk_lib())
-    finally:
-        del os.environ["E264_DBK_DUMP"]
-    assert frames
-    return load_dump(dump)
-
-
 def test_parser_records_deblock_as_the_standard_says(workdir, tmp_path):
     """The stream sets through the parser and the restatement: statement(picture before deblocking) == the deblocked
     picture for every picture.  They include disable_deblocking_filter_idc 2 with slices, filter offsets of +-12, QP 0 and
@@ -377,27 +333,15 @@ def test_parser_records_deblock_as_the_standard_says(workdir, tmp_path):
     assert not zero, zero
 
 
-# the record fuzzer's seeds: seed k takes geometry k % 18 of its list; geometry 14 (120x68) is left to the fuzzer's own
-# comparison with the restatement, the statement takes a minute over it
-FUZZ_SEEDS = [k for k in range(36) if k % 18 != 14]
-
-
 @pytest.fixture(scope="module")
 def fuzzer(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("dbkfuzz") / "record_fuzz")
-    src = [os.path.join(NATIVE, "record_fuzz.c"), os.path.join(ROOT, "oracle", "port_recon.c"), os.path.join(ROOT, "oracle", "record_check.c")]
-    subprocess.run(["gcc", "-O2", "-std=gnu11", "-w", "-pthread"] + src + ["-o", exe, "-ldl"], check=True)
-    return exe
+    return build_fuzzer(str(tmp_path_factory.mktemp("dbkfuzz")))
 
 
 def fuzz_pictures(fuzzer, tmp_path, extra):
     """The fuzzer's dump files and its runs (it compares the device with the restatement itself, and still writes a
     picture that fails that comparison, so that the statement judges it first)."""
-    out = tmp_path / "dump"
-    out.mkdir()
-    runs = [subprocess.run([fuzzer, "--seeds", f"{a}-{b}", "--dump", str(out)] + extra, capture_output=True, text=True, timeout=900)
-            for a, b in ((0, 13), (15, 31), (33, 35))]
-    files = sorted(glob.glob(str(out / "seed_*.bin")), key=lambda f: int(re.search(r"seed_(\d+)", f).group(1)))
+    files, runs = run_fuzzer(fuzzer, str(tmp_path / "dump"), FUZZ_SEEDS, extra)
     assert [int(re.search(r"seed_(\d+)", f).group(1)) for f in files] == FUZZ_SEEDS
     return files, runs
 
