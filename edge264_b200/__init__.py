@@ -47,6 +47,7 @@ class Edge264PicStats(ctypes.Structure):
 
 
 SKIP_NONE, SKIP_NONREF, SKIP_NONKEY = 0, 1, 2   # include/edge264_skip.h
+LOOP_FILTER_ALL, LOOP_FILTER_REF, LOOP_FILTER_NONE = 0, 1, 2   # include/edge264_loopfilter.h
 
 
 _loaded = {}
@@ -85,6 +86,8 @@ def bind(path):
         lib.edge264_set_skip.argtypes = [ctypes.c_void_p, ctypes.c_int]
     if hasattr(lib, "edge264_enable_luma_only"):   # the extension of include/edge264_luma.h
         lib.edge264_enable_luma_only.argtypes = [ctypes.c_void_p]
+    if hasattr(lib, "edge264_set_loop_filter"):   # the extension of include/edge264_loopfilter.h
+        lib.edge264_set_loop_filter.argtypes = [ctypes.c_void_p, ctypes.c_int]
     if hasattr(lib, "edge264_get_picstats"):   # the extension of include/edge264_picstats.h
         lib.edge264_enable_picstats.argtypes = [ctypes.c_void_p]
         lib.edge264_get_picstats.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264PicStats)]
@@ -188,7 +191,7 @@ def frame_picstats(lib, dec, f):
     return out
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False, picstats=False):
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False, picstats=False, loop_filter=LOOP_FILTER_ALL):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
@@ -196,7 +199,8 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
     output (frame_packed); resized=(format, width, height) does the same with the resized output (edge264_enable_resized,
     log2_scale -1); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip); luma_only=True decodes
     the Y plane only, chroma comes out as 128 (edge264_enable_luma_only); picstats=True appends the frame's statistics
-    (frame_picstats) as the last element of each frame tuple."""
+    (frame_picstats) as the last element of each frame tuple; loop_filter=LOOP_FILTER_REF / LOOP_FILTER_NONE outputs
+    the non-reference / all pictures without deblocking (edge264_set_loop_filter)."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -235,6 +239,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             d = ctypes.c_void_p(dec)
             lib.edge264_free(ctypes.byref(d))
             raise RuntimeError("edge264_enable_luma_only: %s" % errno.errorcode.get(r, r))
+    if loop_filter != LOOP_FILTER_ALL:
+        r = lib.edge264_set_loop_filter(dec, loop_filter) if hasattr(lib, "edge264_set_loop_filter") else errno.ENOTSUP
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_set_loop_filter: %s" % errno.errorcode.get(r, r))
     if picstats:
         r = lib.edge264_enable_picstats(dec) if hasattr(lib, "edge264_enable_picstats") else errno.ENOTSUP
         if r:

@@ -161,6 +161,7 @@ typedef struct PicBuild {
 	E264SliceRec *slices; int n_slices;
 	uint32_t *intra_list; int staging;
 	int mbs_done, n_intra, any_deblock; uint16_t slice_counter;
+	int no_deblock;           /* the picture is output without the loop filter (edge264_loopfilter.h): its records are those of deblock idc 1 */
 	int slot, host_buf, conceal_ref;
 	int any_err;              /* some record has err != 0 (a slice error, a missing reference, concealment) */
 	int32_t slot_ids[E264_MAX_SLOTS];   /* FrameId held by every frame slot when the picture started (Pic.slot_uid): the motion export's table */
@@ -212,6 +213,7 @@ struct Edge264Decoder {
 	int cur_idr, cur_nal_ref_idc;
 	int cur_skip;                      /* the current picture is skipped: its headers run, its slice data is dropped */
 	int skip_mode;                     /* edge264_set_skip: applied to each picture at its first slice */
+	int loop_filter_mode;              /* edge264_set_loop_filter: applied to each picture at its first slice */
 	int prev_ref_frame_num, prev_ref_poc;   /* frame_num and POC of the previous reference picture (8.2.1) */
 	int q_prev_ref_frame_num, q_cur_frame_num;   /* reference-style absolute frame numbers, only used to number FrameIds like it */
 	int32_t next_uid;

@@ -20,6 +20,7 @@
 #include "../../include/edge264_picstats.h"
 #include "../../include/edge264_skip.h"
 #include "../../include/edge264_luma.h"
+#include "../../include/edge264_loopfilter.h"
 
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
@@ -1038,7 +1039,11 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 	for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = d->pics[i].in_use ? d->pics[i].uid : -1;
 	if (skip) {   /* no build, no staging: a non-existing frame whose slot is filled if a decoded picture ever predicts from it */
 		cp->nonexisting = 1; cp->unfilled = nal_ref_idc != 0;
-	} else if ((ret = start_build(d, slot, hbuf))) return ret;
+	} else {
+		if ((ret = start_build(d, slot, hbuf))) return ret;
+		/* edge264_loopfilter.h: decided once, at the picture's first slice, like the skip decision */
+		d->pb->no_deblock = d->loop_filter_mode == EDGE264_LOOP_FILTER_NONE || (d->loop_filter_mode == EDGE264_LOOP_FILTER_REF && !nal_ref_idc);
+	}
 
 	/* IDR / MMCO5: every earlier picture leaves in output order first (reference headers.c:632, 680) */
 	int has_mmco5 = 0;
@@ -1102,10 +1107,13 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 	Pic *cp = &d->pics[d->cur];
 	if (h->first_mb >= d->w_mbs * d->h_mbs) return EBADMSG;
 
+	/* a picture without the loop filter (edge264_loopfilter.h) gets the records of disable_deblocking_filter_idc 1; its
+	 * header keeps the values it was parsed with */
+	const int deblock_idc = pb->no_deblock ? 1 : h->deblock_idc;
 	E264SliceRec *sr = &pb->slices[pb->n_slices];
 	memset(sr, 0, sizeof(*sr));
-	sr->filter_offset_a = (int8_t)h->filter_offset_a; sr->filter_offset_b = (int8_t)h->filter_offset_b;
-	sr->deblock_idc = (uint8_t)h->deblock_idc; sr->slice_type = (uint8_t)h->slice_type;
+	if (deblock_idc != 1) { sr->filter_offset_a = (int8_t)h->filter_offset_a; sr->filter_offset_b = (int8_t)h->filter_offset_b; }
+	sr->deblock_idc = (uint8_t)deblock_idc; sr->slice_type = (uint8_t)h->slice_type;
 	merge_scaling(s, p, sr);
 
 	SliceCtx *c = &job->sc;
@@ -1116,7 +1124,7 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 	c->num_ref[0] = h->num_ref[0]; c->num_ref[1] = h->num_ref[1];
 	c->direct_spatial = h->direct_spatial; c->direct_8x8_inference = s->direct_8x8_inference; c->transform_8x8_mode = p->transform_8x8_mode;
 	c->qp = h->slice_qp; c->chroma_qp_offset[0] = p->chroma_qp_index_offset[0]; c->chroma_qp_offset[1] = p->chroma_qp_index_offset[1];
-	c->deblock_idc = h->deblock_idc; c->cur_poc = cp->poc_dec;
+	c->deblock_idc = deblock_idc; c->cur_poc = cp->poc_dec;
 	c->mbi = pb->mbi; c->recs = pb->recs; c->coefs = pb->coefs; c->coef_cap = pb->coef_cap;   /* n_coefs: build_work continues the pool where the previous slice ended */
 	c->col_recs = NULL; c->col_slot_uid = NULL; c->error = 0; c->n_intra = 0; c->missing_ref = 0; c->any_err = 0; c->luma_only = d->luma_only;
 	memset(c->ref_slot, -1, sizeof(c->ref_slot)); memset(c->ref_long, 0, sizeof(c->ref_long));
@@ -1157,7 +1165,7 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 		if (wp == 2) implicit_weights(c, sr);
 	}
 	pb->n_slices++;
-	if (h->deblock_idc != 1) pb->any_deblock = 1;
+	if (deblock_idc != 1) pb->any_deblock = 1;
 
 	c->br = *b;
 	c->mbaddr = h->first_mb;
@@ -1464,5 +1472,14 @@ int edge264_enable_luma_only(Edge264Decoder *d) {
 	if (!d) return EINVAL;
 	if (d->slices_seen) return EBUSY;   /* the pictures of one stream are all decoded one way */
 	d->luma_only = 1;
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* skipping the loop filter (include/edge264_loopfilter.h)                                      */
+/* ------------------------------------------------------------------------------------------ */
+int edge264_set_loop_filter(Edge264Decoder *d, int mode) {
+	if (!d || mode < EDGE264_LOOP_FILTER_ALL || mode > EDGE264_LOOP_FILTER_NONE) return EINVAL;
+	d->loop_filter_mode = mode;   /* read by start_picture only: the current picture keeps its decision */
 	return 0;
 }

@@ -10,6 +10,10 @@
  *
  *   gen264 -o out.264 [-W mbs] [-H mbs] [-n frames] [-s seed] [--cavlc] [--gop I|IP|IPB] [--idr N]
  *          [--refs N] [--t8x8 pct] [--scaling 0|1|2] [--wp 0|1|2] [--slices N] [--deblock 0|1|2]
+ *          [--deblock-off nonref|all]       (disable_deblocking_filter_idc = 1 in the slices of the non-reference / all
+ *                                           pictures; every other bit of the stream, slice data included, is the one
+ *                                           written without the option: the twin of a decode that skips the loop filter,
+ *                                           include/edge264_loopfilter.h)
  *          [--density pct] [--qp Q] [--temporal] [--pcm permille] [--crop-bottom px] [--level idc]
  *          [--mvrange qpel] [--intra-pct P] [--skip-pct P]
  *          [--crop-left px] [--crop-right px] [--crop-top px]   (even numbers; with --crop-bottom: frame cropping rectangle)
@@ -59,6 +63,7 @@ typedef struct GenState {
 	int drift[2];           /* per-picture global motion */
 	int cur_is_b;
 	int i_period;
+	int deblock_off;        /* --deblock-off: 0 none, 1 non-reference pictures, 2 all pictures */
 	int direct4x4, nonref_p, extra_nals, bref, crop_left, crop_right, crop_top, mixed, ps_update, dpb_mode, mmco5, poc_type, max_long_idx_plus1, stat_rplm, stat_mmco[7], stat_idr_long;   /* --dpb: list modification + memory-management stress on I P P P streams; --poc-type 0|1|2 */
 	int wp_full, qp_walk, cqp_fixed, cqp[2], levels_big, pcm_extreme;   /* the standard's limits (file header) */
 } GenState;
@@ -549,8 +554,12 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 		int pic_init_qp = g->qp0;
 		bw_se(&w, slice_qp - pic_init_qp);
 		int idc = g->deblock;
-		bw_ue(&w, idc);
-		if (idc != 1) { bw_se(&w, rnd(g, 13) - 6); bw_se(&w, rnd(g, 13) - 6); }
+		const int off = g->deblock_off == 2 || (g->deblock_off == 1 && !pp->is_ref);
+		bw_ue(&w, off ? 1 : idc);
+		if (idc != 1) {   /* the offsets are drawn either way, so that the rest of the stream does not change */
+			const int a = rnd(g, 13) - 6, b = rnd(g, 13) - 6;
+			if (!off) { bw_se(&w, a); bw_se(&w, b); }
+		}
 
 		/* slice data through the shared writer */
 		SliceCtx *s = (SliceCtx *)calloc(1, sizeof(SliceCtx));
@@ -646,6 +655,10 @@ int main(int argc, char **argv) {
 	g->direct4x4 = argf(argc, argv, "--direct4x4"); g->nonref_p = argf(argc, argv, "--nonref-p"); g->extra_nals = argf(argc, argv, "--extra-nals");
 	g->bref = argf(argc, argv, "--bref");
 	g->i_period = argi(argc, argv, "--i-period", 0);
+	for (int i = 1; i + 1 < argc; i++) if (!strcmp(argv[i], "--deblock-off")) {
+		g->deblock_off = !strcmp(argv[i + 1], "nonref") ? 1 : !strcmp(argv[i + 1], "all") ? 2 : -1;
+		if (g->deblock_off < 0) { fprintf(stderr, "gen264: --deblock-off takes nonref or all\n"); return 2; }
+	}
 	g->mixed = argf(argc, argv, "--mixed-slices"); g->ps_update = argf(argc, argv, "--ps-update");
 	g->dpb_mode = argf(argc, argv, "--dpb"); g->mmco5 = argf(argc, argv, "--mmco5"); g->poc_type = argi(argc, argv, "--poc-type", 0);
 	g->log2_max_frame_num = g->dpb_mode ? 4 : 8; g->log2_max_poc_lsb = 10;
