@@ -91,15 +91,18 @@ def bind(path):
     if hasattr(lib, "edge264_get_picstats"):   # the extension of include/edge264_picstats.h
         lib.edge264_enable_picstats.argtypes = [ctypes.c_void_p]
         lib.edge264_get_picstats.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264PicStats)]
+    if hasattr(lib, "edge264_get_second_view"):   # the extension of include/edge264_mvc.h
+        lib.edge264_get_second_view.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264Frame)]
     _loaded[path] = lib
     return lib
 
 
-def _frame_bytes(f):
+def _frame_bytes(f, mvc=False):
+    """The frame's cropped samples as I420 bytes; mvc=True: those of samples_mvc (the second view of a stereo frame)."""
     out = bytearray()
     for pl in range(3):
         w = f.width_C if pl else f.width_Y; h = f.height_C if pl else f.height_Y; st = f.stride_C if pl else f.stride_Y
-        base = ctypes.cast(f.samples[pl], ctypes.c_void_p).value
+        base = ctypes.cast((f.samples_mvc if mvc else f.samples)[pl], ctypes.c_void_p).value
         for y in range(h):
             out += ctypes.string_at(base + y * st, w)
     return bytes(out)
@@ -191,7 +194,20 @@ def frame_picstats(lib, dec, f):
     return out
 
 
-def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False, picstats=False, loop_filter=LOOP_FILTER_ALL):
+def frame_second_view(lib, dec, f):
+    """The second view of stereo frame f (just returned by edge264_get_frame) as a frame of its own
+    (edge264_get_second_view), or None for a single-view frame."""
+    out = Edge264Frame()
+    r = lib.edge264_get_second_view(dec, ctypes.byref(f), ctypes.byref(out))
+    if r == errno.ENOENT:
+        return None
+    if r:
+        raise RuntimeError("edge264_get_second_view: %s" % errno.errorcode.get(r, r))
+    return out
+
+
+def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False, picstats=False, loop_filter=LOOP_FILTER_ALL,
+                 second_view=False):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
@@ -200,7 +216,10 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
     log2_scale -1); skip=SKIP_NONREF / SKIP_NONKEY leaves those pictures out (edge264_set_skip); luma_only=True decodes
     the Y plane only, chroma comes out as 128 (edge264_enable_luma_only); picstats=True appends the frame's statistics
     (frame_picstats) as the last element of each frame tuple; loop_filter=LOOP_FILTER_REF / LOOP_FILTER_NONE outputs
-    the non-reference / all pictures without deblocking (edge264_set_loop_filter)."""
+    the non-reference / all pictures without deblocking (edge264_set_loop_filter); second_view=True appends the second
+    view of a stereo frame (include/edge264_mvc.h), None for a single-view frame, else a tuple laid out like the frame
+    tuple itself (FrameId_mvc, width, height, i420_bytes and the same optional elements).  A library without
+    edge264_get_second_view (the reference's) gives the second view's FrameId, size and samples only."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -260,10 +279,19 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
         res = lib.edge264_decode_NAL(dec, nal, sc, None, None)
         if nal >= end:
             drained = True
+        def entry(f):
+            return ((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ())
+                    + ((frame_motion(lib, dec, f),) if motion else ()) + ((frame_packed(lib, dec, f),) if packed is not None or resized is not None else ())
+                    + ((frame_picstats(lib, dec, f),) if picstats else ()))
         while lib.edge264_get_frame(dec, ctypes.byref(f), 0) == 0:
-            frames.append((f.FrameId, f.width_Y, f.height_Y, _frame_bytes(f)) + ((_frame_errors(f),) if errors else ())
-                          + ((frame_motion(lib, dec, f),) if motion else ()) + ((frame_packed(lib, dec, f),) if packed is not None or resized is not None else ())
-                          + ((frame_picstats(lib, dec, f),) if picstats else ()))
+            fr = entry(f)
+            if second_view:
+                if hasattr(lib, "edge264_get_second_view"):
+                    sv = frame_second_view(lib, dec, f)
+                    fr += (entry(sv) if sv is not None else None,)
+                else:
+                    fr += ((f.FrameId_mvc, f.width_Y, f.height_Y, _frame_bytes(f, True)) if f.samples_mvc[0] else None,)
+            frames.append(fr)
         if res == errno.ENOBUFS:
             if len(frames) == before:
                 break

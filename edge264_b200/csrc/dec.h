@@ -12,7 +12,8 @@
 #include "cabac.h"
 #include "../../include/edge264.h"
 
-#define E264_MAX_SLOTS   20       /* device frame slots: 16 references + current + slack */
+#define E264_MAX_SLOTS   32       /* device frame slots: two views of up to 15 references (the width of taint, ref_mask and slot_ids) */
+#define E264_MONO_SLOTS  20       /* cap of a single-view sequence: 16 references + current + slack */
 #define E264_MAX_SLICES  64       /* slices per picture (slice_idx is a byte; more are rejected) */
 #define E264_MAX_PPS     16
 
@@ -91,6 +92,8 @@ typedef struct Pic {
 	int poc_dec, poc_top_dec; /* the values in force while the picture itself is decoded: memory_management_control_operation 5 rebases
 	                           * poc/poc_top for output and later pictures only (8.2.1; reference headers.c:46-49, 673-680) */
 	int32_t uid;              /* unique id of the picture = FrameId */
+	int view;                 /* 0 base view, 1 second view of a stereo sequence (edge264_mvc.h) */
+	int ref_frame;            /* the frame the reference decoder would hold the picture in (Edge264Decoder.ref_frame_view) */
 	int nonexisting;
 	int unfilled;             /* a skipped reference picture whose slot has not been filled yet (edge264_skip.h) */
 	E264MbRec *recs;          /* pinned host records of this picture (kept: co-located info for B direct) */
@@ -194,6 +197,7 @@ typedef struct HostBuf {
 	int borrowed;
 	int32_t frame_id;
 	uint64_t ticket;      /* backend completion ticket of the picture written into it */
+	int ref_frame;        /* Pic.ref_frame of the picture in it */
 	int submitted;        /* reconstruction has been enqueued (ticket valid) */
 } HostBuf;
 #define E264_MAX_HOSTBUFS 64
@@ -204,6 +208,8 @@ struct Edge264Decoder {
 	const struct E264Backend *be; void *be_ctx;
 	/* parameter sets */
 	SPS sps; PPS pps[E264_MAX_PPS];
+	SPS ssps;                          /* subset SPS of the second view, valid while mvc */
+	int mvc;                           /* stereo: a subset SPS was accepted; off again at End of sequence and flush (edge264_mvc.h) */
 	/* geometry of the active sequence */
 	int configured, w_mbs, h_mbs, stride_y, stride_c, plane_y, plane_c, frame_bytes, n_slots;
 	Edge264Frame out_fmt;
@@ -211,11 +217,24 @@ struct Edge264Decoder {
 	Pic pics[E264_MAX_SLOTS];
 	int cur;                           /* slot of the picture being decoded, -1 none */
 	int cur_idr, cur_nal_ref_idc;
+	/* Each view keeps its own DPB: the helpers below work on the pictures of d->view, the view of the picture being started
+	 * or finished (the reference's same_views mask, edge264_headers.c:61-100) */
+	int view;
+	int base_slot;                     /* the last base view picture: the second view's inter-view reference, kept in its slot until the next one */
+	int inter_view_flag;               /* of the last prefix NAL unit: the base view component that follows is an inter-view reference */
+	int au_skip;                       /* the skip decision of the access unit's base view, which its second view follows */
+	/* The reference decoder counts a picture just inserted in the DPB towards its view's max_num_reorder_frames only when
+	 * the last picture of its frame buffer was of the same view (its view mask is taken before the picture joins it,
+	 * edge264_headers.c:971, 1160, 1249).  Which frame buffer that is follows from its allocation rule (the lowest one
+	 * holding no reference, no picture waiting for output, none queued or borrowed) and is tracked here so that second views
+	 * leave at the same decode_NAL calls as there.  A single-view stream always counts its picture. */
+	uint8_t ref_frame_view[32];
+	int ghost_frames;                  /* non-existing frames the reference inserts before the current picture (number_frame_id) */
 	int cur_skip;                      /* the current picture is skipped: its headers run, its slice data is dropped */
 	int skip_mode;                     /* edge264_set_skip: applied to each picture at its first slice */
 	int loop_filter_mode;              /* edge264_set_loop_filter: applied to each picture at its first slice */
-	int prev_ref_frame_num, prev_ref_poc;   /* frame_num and POC of the previous reference picture (8.2.1) */
-	int q_prev_ref_frame_num, q_cur_frame_num;   /* reference-style absolute frame numbers, only used to number FrameIds like it */
+	int prev_ref_frame_num[2], prev_ref_poc[2];   /* per view: frame_num and POC of the previous reference picture (8.2.1) */
+	int q_prev_ref_frame_num[2], q_cur_frame_num;   /* reference-style absolute frame numbers, only used to number FrameIds like it */
 	int32_t next_uid;
 	SliceHeader sh;                    /* header of the slice being parsed */
 	SliceHeader first_sh;              /* header of the first slice of the current picture (marking) */
@@ -235,8 +254,8 @@ struct Edge264Decoder {
 	PicBuild *slot_build[E264_MAX_SLOTS]; uint64_t slot_build_seq[E264_MAX_SLOTS];
 	/* output */
 	HostBuf hb[E264_MAX_HOSTBUFS];
-	int outq[E264_MAX_HOSTBUFS]; int outq_n;
-	int pending_release;               /* host buffer handed out without borrow, released at next decode_NAL */
+	int outq[2][E264_MAX_HOSTBUFS]; int outq_n[2];   /* per view; a stereo frame pairs the heads of both */
+	int pending_release[2];            /* host buffers handed out without borrow, released at next decode_NAL */
 	int sync_output;                   /* E264_SYNC_OUTPUT=1: get_frame always waits for the device (the behaviour before round 2's last step; A/B switch) */
 	int motion;                        /* edge264_enable_motion: every output picture carries its motion export */
 	int slices_seen;                   /* a slice NAL unit has been decoded (edge264_enable_motion / _packed / _resized / _picstats are refused from then on) */

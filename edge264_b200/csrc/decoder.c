@@ -21,6 +21,7 @@
 #include "../../include/edge264_skip.h"
 #include "../../include/edge264_luma.h"
 #include "../../include/edge264_loopfilter.h"
+#include "../../include/edge264_mvc.h"
 
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
@@ -105,7 +106,39 @@ static void skip_hrd(BitReader *b) {
 	br_u(b, 20);
 }
 
-static int parse_sps(Edge264Decoder *d, BitReader *b, SPS *out) {
+/* mvc_vui_parameters_extension (H.14.1): walked over, like the reference (headers.c:1699-1736) */
+static void skip_mvc_vui(BitReader *b) {
+	for (int i = br_ue_i(b, 1023); i-- >= 0 && !b->overrun;) {
+		br_u(b, 3);
+		for (int j = br_ue_i(b, 1023); j >= 0 && !b->overrun; j--) br_ue(b);
+		if (br_u1(b)) { br_u(b, 32); br_u(b, 32); br_u1(b); }
+		int nal_hrd = br_u1(b); if (nal_hrd) skip_hrd(b);
+		int vcl_hrd = br_u1(b); if (vcl_hrd) skip_hrd(b);
+		if (nal_hrd || vcl_hrd) br_u1(b);
+		br_u1(b);
+	}
+}
+
+/* seq_parameter_set_mvc_extension (H.7.3.2.1.4): exactly two views; the inter-view references it lists are ignored, the
+ * second view always predicts from its base (reference headers.c:1743-1790).  0 or ENOTSUP. */
+static int parse_sps_mvc_extension(BitReader *b, int profile_idc) {
+	int num_views = br_ue_i(b, 1023) + 1;
+	for (int i = 0; i < num_views && !b->overrun; i++) br_ue(b);
+	if (num_views != 2) return ENOTSUP;
+	for (int k = 0; k < 4; k++) if (br_ue_i(b, 2)) br_ue(b);   /* anchor l0/l1, then non-anchor l0/l1 references of view 1 */
+	for (int i = br_ue_i(b, 63); i >= 0 && !b->overrun; i--) {   /* level values and their operation points */
+		br_u(b, 8);
+		for (int j = br_ue_i(b, 1023); j >= 0 && !b->overrun; j--) {
+			br_u(b, 3);
+			for (int k = br_ue_i(b, 1023); k >= 0 && !b->overrun; k--) br_ue(b);
+			br_ue(b);
+		}
+	}
+	return profile_idc == 134 ? ENOTSUP : 0;   /* MFC High */
+}
+
+/* subset: a subset sequence parameter set (NAL unit 15), whose MVC extension follows the SPS data */
+static int parse_sps(Edge264Decoder *d, BitReader *b, SPS *out, int subset) {
 	SPS s; memset(&s, 0, sizeof(s));
 	int ret = 0;
 	memset(s.sl4x4, 16, sizeof(s.sl4x4)); memset(s.sl8x8, 16, sizeof(s.sl8x8));
@@ -179,6 +212,14 @@ static int parse_sps(Edge264Decoder *d, BitReader *b, SPS *out) {
 			s.max_dec_frame_buffering = buffering > s.max_num_ref_frames ? buffering : s.max_num_ref_frames;
 			s.max_num_reorder_frames = reorder < s.max_dec_frame_buffering ? reorder : s.max_dec_frame_buffering;
 		}
+	}
+	if (subset) {   /* Multiview High and Stereo High only (reference headers.c:2002-2009) */
+		if (s.profile_idc != 118 && s.profile_idc != 128 && s.profile_idc != 134) return ENOTSUP;
+		br_u1(b);   /* bit_equal_to_one */
+		int r = parse_sps_mvc_extension(b, s.profile_idc);
+		if (r) return r;
+		if (br_u1(b)) skip_mvc_vui(b);
+		br_u1(b);   /* additional_extension2_flag */
 	}
 	if (b->overrun) return EBADMSG;
 	(void)d;
@@ -324,39 +365,42 @@ static int hostbuf_acquire(Edge264Decoder *d) {
 }
 static void hostbufs_free_all(Edge264Decoder *d) {
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) hostbuf_free(d, &d->hb[i]);
-	d->outq_n = 0; d->pending_release = -1;
+	d->outq_n[0] = d->outq_n[1] = 0; d->pending_release[0] = d->pending_release[1] = -1;
 }
 
 /* DPB bookkeeping mirrors the reference's bit sets (edge264_internal.h:1217-1222):
  *   ref            <-> prev_short_term_frames / prev_long_term_frames
  *   needed_for_output <-> to_get_frames & ~output_frames */
+/* slot i holds a picture of the view being worked on (d->view) */
+static inline int in_view(const Edge264Decoder *d, int i) { return d->pics[i].in_use && d->pics[i].view == d->view; }
+static inline const SPS *view_sps(const Edge264Decoder *d) { return d->view ? &d->ssps : &d->sps; }
 static int dpb_fullness(Edge264Decoder *d) {
 	int n = 0;
-	for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && (d->pics[i].ref || d->pics[i].needed_for_output)) n++;
+	for (int i = 0; i < d->n_slots; i++) if (in_view(d, i) && (d->pics[i].ref || d->pics[i].needed_for_output)) n++;
 	return n;
 }
 static int waiting_for_output(Edge264Decoder *d) {
 	int n = 0;
-	for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && d->pics[i].needed_for_output) n++;
+	for (int i = 0; i < d->n_slots; i++) if (in_view(d, i) && d->pics[i].needed_for_output) n++;
 	return n;
 }
 static void slot_release_if_unused(Edge264Decoder *d, int i) {
 	Pic *p = &d->pics[i];
-	if (p->in_use && !p->ref && !p->needed_for_output && i != d->cur) p->in_use = 0;
+	if (p->in_use && !p->ref && !p->needed_for_output && i != d->cur && i != d->base_slot) p->in_use = 0;
 }
-/* bumping: output the waiting picture with the lowest POC (reference bump_frame, headers.c:78-95) */
-static int bump_frame(Edge264Decoder *d, int ignore_slot) {
+/* bumping: output the waiting picture of `view` with the lowest POC (reference bump_frame, headers.c:78-95) */
+static int bump_frame(Edge264Decoder *d, int view, int ignore_slot) {
 	int best = -1;
 	for (int i = 0; i < d->n_slots; i++) {
 		Pic *p = &d->pics[i];
-		if (!p->in_use || !p->needed_for_output || i == ignore_slot) continue;
+		if (!p->in_use || p->view != view || !p->needed_for_output || i == ignore_slot) continue;
 		if (best < 0 || p->poc_top < d->pics[best].poc_top) best = i;
 	}
 	if (best < 0) return 0;
 	Pic *p = &d->pics[best];
 	p->needed_for_output = 0;
 	if (p->host_buf >= 0) {
-		d->hb[p->host_buf].state = 2; d->outq[d->outq_n++] = p->host_buf;
+		d->hb[p->host_buf].state = 2; d->outq[view][d->outq_n[view]++] = p->host_buf;
 		if (__atomic_load_n(&d->hb[p->host_buf].submitted, __ATOMIC_ACQUIRE)) p->host_buf = -1;   /* a worker may be submitting it */
 	}
 	slot_release_if_unused(d, best);
@@ -401,7 +445,7 @@ static void conceal_missing(Edge264Decoder *d, PicBuild *pb) {
 /* the frame slot a lost macroblock is copied from: the most recent reference picture (header-time state) */
 static int conceal_reference(Edge264Decoder *d) {
 	int ref = -1, best = -1;
-	for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use && d->pics[i].ref && !d->pics[i].nonexisting && d->pics[i].uid > best) { best = d->pics[i].uid; ref = i; }
+	for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i) && d->pics[i].ref && !d->pics[i].nonexisting && d->pics[i].uid > best) { best = d->pics[i].uid; ref = i; }
 	return ref;
 }
 
@@ -459,6 +503,7 @@ static int finish_picture(Edge264Decoder *d) {
 	if (d->cur < 0) return 0;
 	Pic *p = &d->pics[d->cur];
 	int ret = 0;
+	d->view = p->view;
 	if (d->pb) {   /* a skipped picture has no build */
 		pthread_mutex_lock(&d->lock);
 		d->pb->conceal_ref = conceal_reference(d);
@@ -470,9 +515,11 @@ static int finish_picture(Edge264Decoder *d) {
 	}
 	if (p->host_buf >= 0 && !p->needed_for_output) p->host_buf = -1;   /* already in the output queue */
 	apply_marking(d);
-	int c = d->cur;
+	int c = d->cur, old_base = -1;
 	d->cur = -1;
+	if (d->mvc && !p->view) { old_base = d->base_slot; d->base_slot = c; }   /* the reference's basePic (headers.c:73-74) */
 	slot_release_if_unused(d, c);
+	if (old_base >= 0 && old_base != c) slot_release_if_unused(d, old_base);
 	return ret;
 }
 
@@ -620,7 +667,7 @@ static void apply_marking(Edge264Decoder *d) {
 	if (!d->cur_nal_ref_idc) { cur->ref = 0; return; }
 	int cur_long = 0;
 	if (d->cur_idr) {
-		for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use) { d->pics[i].ref = 0; slot_release_if_unused(d, i); }
+		for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i)) { d->pics[i].ref = 0; slot_release_if_unused(d, i); }
 		cur_long = h->long_term_reference_flag;
 		cur->long_term_idx = 0;
 	} else {
@@ -629,34 +676,34 @@ static void apply_marking(Edge264Decoder *d) {
 			int target = -1;
 			if (op == 1 || op == 3) {
 				int fn = cur->frame_num - 1 - (int)h->mmco[k].a;
-				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use && d->pics[i].ref == 1 && d->pics[i].frame_num == fn) { target = i; d->pics[i].ref = 0; }
+				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i) && d->pics[i].ref == 1 && d->pics[i].frame_num == fn) { target = i; d->pics[i].ref = 0; }
 			}
 			if (op == 2 || op == 3 || op == 4 || op == 6) {
 				int idx = (int)(op == 3 ? h->mmco[k].b : h->mmco[k].a);
 				int up = op == 4 ? INT_MAX : idx;
 				if (op == 4) idx = (int)h->mmco[k].a;   /* max_long_term_frame_idx_plus1: drop idx >= a */
-				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use && d->pics[i].ref == 2 && d->pics[i].long_term_idx >= idx && d->pics[i].long_term_idx <= up) d->pics[i].ref = 0;
+				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i) && d->pics[i].ref == 2 && d->pics[i].long_term_idx >= idx && d->pics[i].long_term_idx <= up) d->pics[i].ref = 0;
 				if (op == 3 && target >= 0) { d->pics[target].ref = 2; d->pics[target].long_term_idx = idx; }
 				if (op == 6) { cur_long = 1; cur->long_term_idx = idx; }
 			}
 			if (op == 5) {
-				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use) d->pics[i].ref = 0;
+				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i)) d->pics[i].ref = 0;
 			}
 		}
 		for (int i = 0; i < d->n_slots; i++) slot_release_if_unused(d, i);
 	}
 	int nref = 0;
-	for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use && d->pics[i].ref) nref++;
-	if (nref >= d->sps.max_num_ref_frames) {
+	for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i) && d->pics[i].ref) nref++;
+	if (nref >= view_sps(d)->max_num_ref_frames) {
 		int best = -1;
-		for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use && d->pics[i].ref == 1 && (best < 0 || d->pics[i].frame_num < d->pics[best].frame_num)) best = i;
+		for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i) && d->pics[i].ref == 1 && (best < 0 || d->pics[i].frame_num < d->pics[best].frame_num)) best = i;
 		if (best >= 0) { d->pics[best].ref = 0; slot_release_if_unused(d, best); }
 	}
 	cur->ref = cur_long ? 2 : 1;
 	for (int k = 0; k < h->n_mmco; k++) if (h->mmco[k].op == 5) cur->frame_num = 0;   /* 8.2.1: the picture is now "frame_num 0" for everything that follows */
-	d->prev_ref_frame_num = cur->frame_num;
-	d->q_prev_ref_frame_num = d->q_cur_frame_num;
-	for (int k = 0; k < h->n_mmco; k++) if (h->mmco[k].op == 5) d->q_prev_ref_frame_num = 0;
+	d->prev_ref_frame_num[d->view] = cur->frame_num;
+	d->q_prev_ref_frame_num[d->view] = d->q_cur_frame_num;
+	for (int k = 0; k < h->n_mmco; k++) if (h->mmco[k].op == 5) d->q_prev_ref_frame_num[d->view] = 0;
 }
 
 /* ------------------------------------------------------------------------------------------ */
@@ -665,8 +712,8 @@ static void apply_marking(Edge264Decoder *d) {
 static int bump_all(Edge264Decoder *d) {
 	if (d->cur >= 0) finish_picture(d);
 	threads_drain(d, NULL);
-	while (bump_frame(d, -1));
-	if (d->outq_n) return ENOBUFS;
+	for (int v = 0; v < 2; v++) while (bump_frame(d, v, -1));
+	if (d->outq_n[0] || d->outq_n[1]) return ENOBUFS;
 	/* frames the application still holds (borrowed, or handed out until the next decode_NAL) keep their buffers: a
 	 * change of format must wait for them like the reference's `to_get_frames | output_frames` test (headers.c:2005-2007) */
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state == 3 && d->hb[i].borrowed) return ENOBUFS;
@@ -686,9 +733,17 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	d->n_builds = d->n_threads ? d->n_threads + 2 : 1;
 	if (d->n_builds > E264_MAX_BUILDS) d->n_builds = E264_MAX_BUILDS;
 	pthread_mutex_unlock(&d->lock);
-	/* a picture keeps its slot (and the slot's record buffer) until it is handed to the device: parsing ahead needs one spare slot per picture in flight */
-	d->n_slots = s->max_num_ref_frames + 2 + (d->n_threads ? d->n_builds : 0);
-	if (d->n_slots > E264_MAX_SLOTS) d->n_slots = E264_MAX_SLOTS;
+	/* a picture keeps its slot (and the slot's record buffer) until it is handed to the device: parsing ahead needs one spare slot per picture in flight.
+	 * A stereo sequence holds both views' references, current pictures and waiting pictures; past 32 slots it gives up the parse-ahead slack and
+	 * the waiting slots before any reference slot (case 15 refuses views that do not fit). */
+	const int slack = d->n_threads ? d->n_builds : 0;
+	if (!d->mvc) {
+		d->n_slots = s->max_num_ref_frames + 2 + slack;
+		if (d->n_slots > E264_MONO_SLOTS) d->n_slots = E264_MONO_SLOTS;
+	} else {
+		d->n_slots = s->max_num_ref_frames + d->ssps.max_num_ref_frames + 4 + slack;
+		if (d->n_slots > E264_MAX_SLOTS) d->n_slots = E264_MAX_SLOTS;
+	}
 	E264PicDesc g; memset(&g, 0, sizeof(g));
 	g.width_mbs = d->w_mbs; g.height_mbs = d->h_mbs; g.stride_y = d->stride_y; g.stride_c = d->stride_c; g.plane_y = d->plane_y; g.frame_bytes = d->frame_bytes;
 	g.staging = d->n_threads ? (d->n_threads + 2 > E264_MAX_BUILDS ? E264_MAX_BUILDS : d->n_threads + 2) + 2 : 0;   /* staging areas wanted: one per picture being parsed + two in flight on the device; 0 = the backend's default */
@@ -707,7 +762,7 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	if (oom) return ENOMEM;
 	memset(d->pics, 0, sizeof(d->pics));
 	for (int i = 0; i < E264_MAX_SLOTS; i++) d->pics[i].host_buf = -1;
-	d->cur = -1;
+	d->cur = -1; d->base_slot = -1;
 	Edge264Frame *o = &d->out_fmt; memset(o, 0, sizeof(*o));
 	o->bit_depth_Y = o->bit_depth_C = 8;
 	o->width_Y = (int16_t)(w - s->crop[0] - s->crop[1]); o->height_Y = (int16_t)(h - s->crop[2] - s->crop[3]);
@@ -717,7 +772,10 @@ static int configure_sequence(Edge264Decoder *d, const SPS *s, int keep_numberin
 	o->frame_crop_offsets[0] = (int16_t)s->crop[2]; o->frame_crop_offsets[1] = (int16_t)s->crop[1];
 	o->frame_crop_offsets[2] = (int16_t)s->crop[3]; o->frame_crop_offsets[3] = (int16_t)s->crop[0];
 	d->configured = 1;
-	if (!keep_numbering) { d->q_prev_ref_frame_num = -1; d->prev_ref_frame_num = -1; d->prev_ref_poc = 0; }
+	if (!keep_numbering) {
+		for (int v = 0; v < 2; v++) { d->q_prev_ref_frame_num[v] = -1; d->prev_ref_frame_num[v] = -1; d->prev_ref_poc[v] = 0; }
+		memset(d->ref_frame_view, 0, sizeof(d->ref_frame_view));
+	}
 	return 0;
 }
 
@@ -726,8 +784,8 @@ static inline int clamp8(int v) { return v < -128 ? -128 : v > 127 ? 127 : v; } 
 /* ------------------------------------------------------------------------------------------ */
 /* slice header                                                                                 */
 /* ------------------------------------------------------------------------------------------ */
-static int parse_slice_header(Edge264Decoder *d, BitReader *b, int nal_unit_type, int nal_ref_idc, SliceHeader *h, const PPS **ppps) {
-	const SPS *s = &d->sps;
+/* s: the SPS of the slice's view; idr: IdrPicFlag (nal_unit_type 5, or non_idr_flag 0 in a NAL unit 20 header) */
+static int parse_slice_header(Edge264Decoder *d, const SPS *s, BitReader *b, int nal_unit_type, int idr, int nal_ref_idc, SliceHeader *h, const PPS **ppps) {
 	memset(h, 0, sizeof(*h));
 	h->first_mb = br_ue_i(b, 139264);   /* bounded like the reference's get_ue32(139263) (headers.c:968); anything larger fails the first_mb >= total test */
 	int st = br_ue_i(b, 10);
@@ -740,9 +798,9 @@ static int parse_slice_header(Edge264Decoder *d, BitReader *b, int nal_unit_type
 	if (!s->valid || !p->valid) return EBADMSG;
 	*ppps = p;
 	h->frame_num = br_u(b, s->log2_max_frame_num);
-	if (nal_unit_type == 5) h->frame_num = 0;
+	if (idr) h->frame_num = 0;
 	h->idr_pic_id = -1;
-	if (nal_unit_type == 5) h->idr_pic_id = br_ue_i(b, 65536);
+	if (idr) h->idr_pic_id = br_ue_i(b, 65536);
 	if (s->poc_type == 0) {
 		h->poc_lsb = br_u(b, s->log2_max_poc_lsb);
 		if (p->bottom_field_pic_order_present) h->delta_poc_bottom = br_se(b);
@@ -784,7 +842,7 @@ static int parse_slice_header(Edge264Decoder *d, BitReader *b, int nal_unit_type
 		}
 	}
 	if (nal_ref_idc) {
-		if (nal_unit_type == 5) { h->no_output_of_prior_pics = br_u1(b); h->long_term_reference_flag = br_u1(b); }
+		if (idr) { h->no_output_of_prior_pics = br_u1(b); h->long_term_reference_flag = br_u1(b); }
 		else if (br_u1(b)) {
 			h->adaptive_marking = 1;
 			int n = 0;
@@ -824,10 +882,9 @@ static void build_ref_lists(Edge264Decoder *d, const SliceHeader *h, int lists[2
 	int st[E264_MAX_SLOTS], lt[E264_MAX_SLOTS], nst = 0, nlt = 0;
 	for (int l = 0; l < 2; l++) for (int i = 0; i < 32; i++) lists[l][i] = -1;
 	nlist[0] = nlist[1] = 0;
-	if (d->cur_idr) return;
-	for (int i = 0; i < d->n_slots; i++) {
+	for (int i = 0; i < d->n_slots && !d->cur_idr; i++) {
 		Pic *p = &d->pics[i];
-		if (i == d->cur || !p->in_use) continue;
+		if (i == d->cur || !in_view(d, i)) continue;
 		if (p->ref == 1) st[nst++] = i; else if (p->ref == 2) lt[nlt++] = i;
 	}
 	/* long-term by LongTermFrameIdx ascending */
@@ -853,20 +910,23 @@ static void build_ref_lists(Edge264Decoder *d, const SliceHeader *h, int lists[2
 		for (int i = 0; i < nb; i++) lists[1][n++] = before[i];
 		for (int i = 0; i < nlt; i++) lists[1][n++] = lt[i];
 		nlist[1] = n;
-		if (n > 1 && lists[0][0] == lists[1][0]) { int t = lists[1][0]; lists[1][0] = lists[1][1]; lists[1][1] = t; }
 	}
+	/* H.8.2.1: the second view appends its inter-view reference, the base view of its access unit, to both lists (reference
+	 * headers.c:784-792: it keeps its place in the before/after swap) */
+	if (d->view) { lists[0][nlist[0]++] = d->base_slot; if (h->slice_type == 1) lists[1][nlist[1]++] = d->base_slot; }
+	if (h->slice_type == 1 && nlist[1] > 1 && lists[0][0] == lists[1][0]) { int t = lists[1][0]; lists[1][0] = lists[1][1]; lists[1][1] = t; }
 	/* 8.2.4.3 modification */
-	int mask = (1 << d->sps.log2_max_frame_num) - 1;
+	int mask = (1 << view_sps(d)->log2_max_frame_num) - 1;
 	for (int l = 0; l <= (h->slice_type == 1); l++) {
 		int pic_num_pred = cur->frame_num;
 		for (int k = 0; k < h->n_mod[l]; k++) {
 			int op = h->mod[l][k].op, pic = -1;
 			if (op < 2) {
 				pic_num_pred = op == 0 ? pic_num_pred - ((int)h->mod[l][k].val + 1) : pic_num_pred + ((int)h->mod[l][k].val + 1);
-				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use && d->pics[i].ref == 1 && !((d->pics[i].frame_num ^ pic_num_pred) & mask)) { pic = i; break; }
+				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i) && d->pics[i].ref == 1 && !((d->pics[i].frame_num ^ pic_num_pred) & mask)) { pic = i; break; }
 			} else if (op == 2) {
-				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && d->pics[i].in_use && d->pics[i].ref == 2 && d->pics[i].long_term_idx == (int)h->mod[l][k].val) { pic = i; break; }
-			}
+				for (int i = 0; i < d->n_slots; i++) if (i != d->cur && in_view(d, i) && d->pics[i].ref == 2 && d->pics[i].long_term_idx == (int)h->mod[l][k].val) { pic = i; break; }
+			} else if (d->view) pic = d->base_slot;   /* idc 4 and 5 name the one inter-view reference (H.8.2.2.3; reference headers.c:848) */
 			if (pic < 0) continue;
 			if (k >= h->num_ref[l] || k >= 32) break;   /* more operations than list entries: the reference stops at refIdx 32 too (headers.c:817) */
 			int buf = pic, c = k;
@@ -891,10 +951,10 @@ static int find_free_slot(Edge264Decoder *d) {
 
 /* 8.2.1 PicOrderCnt and TopFieldOrderCnt of a frame, from its absolute (unwrapped) frame number */
 static void picture_poc(const Edge264Decoder *d, const SliceHeader *h, int idr, int nal_ref_idc, int frame_num_abs, int *poc, int *poc_top) {
-	const SPS *s = &d->sps;
+	const SPS *s = view_sps(d);
 	if (s->poc_type == 0) {
 		int sh = 32 - s->log2_max_poc_lsb;
-		int prev_poc = idr ? 0 : d->prev_ref_poc;
+		int prev_poc = idr ? 0 : d->prev_ref_poc[d->view];
 		int inc = (int)((unsigned)(h->poc_lsb - prev_poc) << sh) >> sh;
 		*poc = *poc_top = prev_poc + inc;
 		if (h->delta_poc_bottom < 0) *poc += h->delta_poc_bottom;   /* PicOrderCnt = min(top, bottom) */
@@ -915,8 +975,34 @@ static void picture_poc(const Edge264Decoder *d, const SliceHeader *h, int idr, 
 /* short-term frames the DPB has room for: max_num_ref_frames less the long-term frames */
 static int short_term_room(const Edge264Decoder *d) {
 	int nlong = 0;
-	for (int i = 0; i < d->n_slots; i++) nlong += d->pics[i].in_use && d->pics[i].ref == 2;
-	return d->sps.max_num_ref_frames - nlong;
+	for (int i = 0; i < d->n_slots; i++) nlong += in_view(d, i) && d->pics[i].ref == 2;
+	return view_sps(d)->max_num_ref_frames - nlong;
+}
+
+/* the reference decoder's frame buffer for a picture of d->view entering the DPB now (Edge264Decoder.ref_frame_view);
+ * returns whether that buffer last held a picture of the same view */
+static int take_ref_frame(Edge264Decoder *d, Pic *p) {
+	uint32_t busy = 0, dropped = 0;
+	const int ghosts = d->ghost_frames;
+	d->ghost_frames = 0;
+	if (ghosts) {   /* it makes room for them by dropping its view's oldest short-term references first (headers.c:1095-1110) */
+		int excess = -short_term_room(d) + ghosts;
+		for (int i = 0; i < d->n_slots; i++) excess += in_view(d, i) && d->pics[i].ref == 1 && &d->pics[i] != p;
+		while (excess-- > 0) {
+			int old = -1;
+			for (int i = 0; i < d->n_slots; i++) if (in_view(d, i) && d->pics[i].ref == 1 && &d->pics[i] != p && !(dropped >> i & 1) &&
+			                                       (old < 0 || d->pics[i].frame_num < d->pics[old].frame_num)) old = i;
+			if (old >= 0) dropped |= 1u << old;
+		}
+	}
+	for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && ((d->pics[i].ref && !(dropped >> i & 1)) || d->pics[i].needed_for_output)) busy |= 1u << d->pics[i].ref_frame;
+	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state == 2 || (d->hb[i].state == 3 && d->hb[i].borrowed)) busy |= 1u << d->hb[i].ref_frame;
+	for (int k = 0; k < ghosts && busy != ~0u; k++) { const int g = __builtin_ctz(~busy); d->ref_frame_view[g] = (uint8_t)d->view; busy |= 1u << g; }
+	const int f = busy == ~0u ? 0 : __builtin_ctz(~busy);
+	const int same = d->ref_frame_view[f] == d->view;
+	d->ref_frame_view[f] = (uint8_t)d->view; p->ref_frame = f;
+	if (p->host_buf >= 0) d->hb[p->host_buf].ref_frame = f;
+	return same;
 }
 
 /* 8.2.5.2 gaps in frame_num (a reference picture was lost): like the reference (headers.c:1095-1139) insert
@@ -925,26 +1011,27 @@ static int short_term_room(const Edge264Decoder *d) {
  * what the encoder meant.  Their samples are undefined in the reference (never-written buffers); ours are
  * cleared.  Returns the number of frames inserted. */
 static int fill_frame_num_gap(Edge264Decoder *d, int frame_num_abs) {
-	const SPS *s = &d->sps;
-	int prev = d->prev_ref_frame_num;
+	const SPS *s = view_sps(d);
+	int prev = d->prev_ref_frame_num[d->view];
 	if (prev < 0 || frame_num_abs - prev <= 1) return 0;
 	int room = short_term_room(d), nshort = 0;
-	for (int i = 0; i < d->n_slots; i++) nshort += d->pics[i].in_use && d->pics[i].ref == 1;
+	for (int i = 0; i < d->n_slots; i++) nshort += in_view(d, i) && d->pics[i].ref == 1;
 	int gap_frames = frame_num_abs - prev - 1 < room ? frame_num_abs - prev - 1 : room;
 	if (gap_frames < 0) gap_frames = 0;
 	for (; gap_frames + nshort > room && nshort > 0; nshort--) {
 		int old = -1;
-		for (int i = 0; i < d->n_slots; i++) if (d->pics[i].in_use && d->pics[i].ref == 1 && (old < 0 || d->pics[i].frame_num < d->pics[old].frame_num)) old = i;
+		for (int i = 0; i < d->n_slots; i++) if (in_view(d, i) && d->pics[i].ref == 1 && (old < 0 || d->pics[i].frame_num < d->pics[old].frame_num)) old = i;
 		d->pics[old].ref = 0; slot_release_if_unused(d, old);
 	}
 	if (gap_frames > 0) threads_drain(d, NULL);   /* the fills below go straight to the device: every earlier picture must be on its way first */
 	for (int fn = frame_num_abs - gap_frames; fn < frame_num_abs; fn++) {
 		int sl = find_free_slot(d);
-		while (sl < 0 && bump_frame(d, -1)) sl = find_free_slot(d);
+		while (sl < 0 && bump_frame(d, d->view, -1)) sl = find_free_slot(d);
 		if (sl < 0) { d->next_uid++; continue; }   /* no room even after bumping: keep at least the FrameId numbering */
 		Pic *np = &d->pics[sl];
 		memset(np, 0, sizeof(*np));
-		np->in_use = 1; np->ref = 1; np->nonexisting = 1; np->frame_num = fn; np->uid = d->next_uid++; np->host_buf = -1;
+		np->in_use = 1; np->ref = 1; np->nonexisting = 1; np->frame_num = fn; np->uid = d->next_uid++; np->host_buf = -1; np->view = d->view;
+		take_ref_frame(d, np);
 		int npoc = 0;
 		if (s->poc_type == 2) npoc = fn * 2;
 		else if (s->poc_type == 1 && s->num_ref_frames_in_poc_cycle > 0) {
@@ -957,21 +1044,21 @@ static int fill_frame_num_gap(Edge264Decoder *d, int frame_num_abs) {
 		if (d->be->fill_slot) { pthread_mutex_lock(&d->be_lock); d->be->fill_slot(d->be_ctx, sl, 0, d->luma_only ? 128 : 0); pthread_mutex_unlock(&d->be_lock); }
 		d->taint |= 1u << sl;   /* its error map is all 100 */
 	}
-	d->prev_ref_frame_num = frame_num_abs - 1;   /* the last inserted frame is the previous reference frame now (headers.c:1131) */
+	d->prev_ref_frame_num[d->view] = frame_num_abs - 1;   /* the last inserted frame is the previous reference frame now (headers.c:1131) */
 	return gap_frames;
 }
 
 /* FrameId numbering: the reference keeps an absolute FrameNum across IDRs, so an IDR after other pictures looks like a
  * frame_num gap and non-existing frames take FrameIds (headers.c:1059,1095-1139) */
 static void number_frame_id(Edge264Decoder *d, int frame_num, int gap_frames) {
-	int q = d->q_prev_ref_frame_num;
-	int qfn = q + 1 + ((frame_num - q - 1) & ((1 << d->sps.log2_max_frame_num) - 1));
+	int q = d->q_prev_ref_frame_num[d->view];
+	int qfn = q + 1 + ((frame_num - q - 1) & ((1 << view_sps(d)->log2_max_frame_num) - 1));
 	int gap = qfn - q;
 	if (gap > 1 && !gap_frames) {   /* a real gap has just been given its frames (and FrameIds) by fill_frame_num_gap */
 		int room = short_term_room(d), n = gap - 1 < room ? gap - 1 : room;
-		if (n > 0) d->next_uid += n;
+		if (n > 0) { d->next_uid += n; d->ghost_frames = n; }
 	}
-	if (gap > 1) d->q_prev_ref_frame_num = qfn - 1;
+	if (gap > 1) d->q_prev_ref_frame_num[d->view] = qfn - 1;
 	d->q_cur_frame_num = qfn;
 }
 
@@ -1002,38 +1089,43 @@ static int start_build(Edge264Decoder *d, int slot, int hbuf) {
 /* first slice of a picture: frame number, POC, FrameId, slot, the data side (start_build) unless the picture is skipped,
  * bumping; sets d->cur, d->cur_skip */
 static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int nal_ref_idc) {
-	const SPS *s = &d->sps;
+	const SPS *s = view_sps(d);
+	const int v = d->view;
 	int ret;
-	if (d->outq_n > 16) {
+	if (d->outq_n[v] > 16) {
 		/* the frame the application is told to fetch may still be with a parser: wait for it here, not in a polling
 		 * loop (without workers every queued frame has been submitted, so this does not wait) */
 		pthread_mutex_lock(&d->lock);
-		while (!__atomic_load_n(&d->hb[d->outq[0]].submitted, __ATOMIC_ACQUIRE)) pthread_cond_wait(&d->done_cv, &d->lock);
+		while (!__atomic_load_n(&d->hb[d->outq[v][0]].submitted, __ATOMIC_ACQUIRE)) pthread_cond_wait(&d->done_cv, &d->lock);
 		pthread_mutex_unlock(&d->lock);
 		return ENOBUFS;
 	}
-	/* edge264_skip.h: decided once, at the picture's first slice */
-	const int skip = d->skip_mode == EDGE264_SKIP_NONREF ? !nal_ref_idc : d->skip_mode == EDGE264_SKIP_NONKEY ? !idr && h->slice_type != 2 : 0;
+	/* edge264_skip.h: decided once, at the picture's first slice; in a stereo sequence once per access unit, at its base view,
+	 * whose inter_view_flag makes it a reference for NONREF, and the second view follows it */
+	const int reference = nal_ref_idc || (d->mvc && d->inter_view_flag);
+	const int skip = v ? d->au_skip : d->skip_mode == EDGE264_SKIP_NONREF ? !reference : d->skip_mode == EDGE264_SKIP_NONKEY ? !idr && h->slice_type != 2 : 0;
 	int hbuf = -1;
 	if (!skip && (hbuf = hostbuf_acquire(d)) < 0) return ENOBUFS;
+	if (!v) d->au_skip = skip;
 	/* absolute (unwrapped) frame numbers like the reference (headers.c:1059) */
-	int prev = d->prev_ref_frame_num;
+	int prev = d->prev_ref_frame_num[v];
 	int frame_num_abs = idr ? 0 : prev + 1 + ((h->frame_num - prev - 1) & ((1 << s->log2_max_frame_num) - 1));
-	if (idr) { d->prev_ref_frame_num = -1; d->prev_ref_poc = 0; }
+	if (idr) { d->prev_ref_frame_num[v] = -1; d->prev_ref_poc[v] = 0; }
 	int poc, poc_top;
 	picture_poc(d, h, idr, nal_ref_idc, frame_num_abs, &poc, &poc_top);
 	int gap_frames = idr ? 0 : fill_frame_num_gap(d, frame_num_abs);
 
 	int slot = find_free_slot(d);
 	if (slot < 0) {   /* DPB invariant broken (stream exceeds its own limits): drop the oldest output-pending picture */
-		if (!bump_frame(d, -1)) return EBADMSG;
+		if (!bump_frame(d, v, -1)) return EBADMSG;
 		slot = find_free_slot(d);
 		if (slot < 0) return ENOBUFS;
 	}
 	Pic *cp = &d->pics[slot];
 	memset(cp, 0, sizeof(*cp));
 	number_frame_id(d, idr ? 0 : h->frame_num, gap_frames);
-	cp->in_use = 1; cp->frame_num = frame_num_abs; cp->poc = cp->poc_dec = poc; cp->poc_top = cp->poc_top_dec = poc_top; cp->uid = d->next_uid++; cp->host_buf = hbuf;
+	cp->in_use = 1; cp->frame_num = frame_num_abs; cp->poc = cp->poc_dec = poc; cp->poc_top = cp->poc_top_dec = poc_top; cp->uid = d->next_uid++; cp->host_buf = hbuf; cp->view = v;
+	const int counted = take_ref_frame(d, cp);
 	d->cur = slot; d->cur_idr = idr; d->cur_nal_ref_idc = nal_ref_idc; d->cur_skip = skip;
 	d->first_sh = *h;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = d->pics[i].in_use ? d->pics[i].uid : -1;
@@ -1041,32 +1133,33 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 		cp->nonexisting = 1; cp->unfilled = nal_ref_idc != 0;
 	} else {
 		if ((ret = start_build(d, slot, hbuf))) return ret;
-		/* edge264_loopfilter.h: decided once, at the picture's first slice, like the skip decision */
-		d->pb->no_deblock = d->loop_filter_mode == EDGE264_LOOP_FILTER_NONE || (d->loop_filter_mode == EDGE264_LOOP_FILTER_REF && !nal_ref_idc);
+		/* edge264_loopfilter.h: decided once, at the picture's first slice, like the skip decision; for each view component,
+		 * a base view with inter_view_flag counting as a reference */
+		d->pb->no_deblock = d->loop_filter_mode == EDGE264_LOOP_FILTER_NONE || (d->loop_filter_mode == EDGE264_LOOP_FILTER_REF && !(v ? nal_ref_idc : reference));
 	}
 
 	/* IDR / MMCO5: every earlier picture leaves in output order first (reference headers.c:632, 680) */
 	int has_mmco5 = 0;
 	for (int k = 0; k < h->n_mmco; k++) if (h->mmco[k].op == 5) has_mmco5 = 1;
 	if (idr || has_mmco5) {
-		while (bump_frame(d, slot));
+		while (bump_frame(d, v, slot));
 		if (has_mmco5) { cp->poc_top -= cp->poc; cp->poc = 0; }   /* tempPicOrderCnt subtraction (8.2.1) for output order and later pictures; frame_num restarts in apply_marking, once the picture's own lists and operations have used the real value */
 	}
 	/* C.4.5.3 bumping before insertion (reference headers.c:1229-1250) */
 	int max_bump = s->max_num_ref_frames;
 	if (!nal_ref_idc) {
 		max_bump = 0;
-		for (int i = 0; i < d->n_slots; i++) if (i != slot && d->pics[i].in_use && d->pics[i].needed_for_output && d->pics[i].poc_top < cp->poc_top) max_bump++;
+		for (int i = 0; i < d->n_slots; i++) if (i != slot && in_view(d, i) && d->pics[i].needed_for_output && d->pics[i].poc_top < cp->poc_top) max_bump++;
 	}
-	while (dpb_fullness(d) >= s->max_dec_frame_buffering && max_bump--) bump_frame(d, slot);
+	while (dpb_fullness(d) >= s->max_dec_frame_buffering && max_bump--) bump_frame(d, v, slot);
 	cp->needed_for_output = 1;   /* a skipped picture too: it leaves by bumping as in a full decode, without a buffer to queue */
 	if (max_bump < 0) {   /* nothing may precede it: straight to the output queue (it is returned once decoded) */
 		cp->needed_for_output = 0;
-		if (!skip) { d->hb[hbuf].state = 2; d->outq[d->outq_n++] = hbuf; }
-	} else if (waiting_for_output(d) > s->max_num_reorder_frames) bump_frame(d, -1);
+		if (!skip) { d->hb[hbuf].state = 2; d->outq[v][d->outq_n[v]++] = hbuf; }
+	} else if (waiting_for_output(d) - !counted > s->max_num_reorder_frames) bump_frame(d, v, -1);
 	/* POC bookkeeping for the next picture (8.2.1.1) */
-	if (nal_ref_idc) { d->prev_ref_poc = has_mmco5 ? cp->poc_top : poc_top; }
-	if (has_mmco5) d->prev_ref_frame_num = 0;
+	if (nal_ref_idc) { d->prev_ref_poc[v] = has_mmco5 ? cp->poc_top : poc_top; }
+	if (has_mmco5) d->prev_ref_frame_num[v] = 0;
 	return 0;
 }
 
@@ -1101,7 +1194,7 @@ static void fill_skipped(Edge264Decoder *d, int slot) {
 
 /* slice record (deblocking, weights, scaling lists) and parsing context (reference lists, co-located slot in *col_slot) */
 static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, const BitReader *b, SliceJob *job, int *col_slot) {
-	const SPS *s = &d->sps;
+	const SPS *s = view_sps(d);
 	PicBuild *pb = d->pb;
 	if (pb->n_slices >= E264_MAX_SLICES) return ENOTSUP;
 	Pic *cp = &d->pics[d->cur];
@@ -1175,22 +1268,24 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 
 /* Parses the slice header, starts a picture when it is the first slice of one and queues the slice's data on the
  * picture's build.  *jobp is set to NULL once the job is queued; until then it stays the caller's. */
-static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, BitReader *b, SliceJob **jobp) {
+static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, int view, int idr, BitReader *b, SliceJob **jobp) {
 	SliceHeader *h = &d->sh;
 	const PPS *p = NULL;
-	int ret = parse_slice_header(d, b, nal_unit_type, nal_ref_idc, h, &p);
+	const SPS *s = view ? &d->ssps : &d->sps;
+	int ret = parse_slice_header(d, s, b, nal_unit_type, idr, nal_ref_idc, h, &p);
 	if (ret) return ret;
-	const SPS *s = &d->sps;
 	if (!d->configured) return EBADMSG;
 
-	/* 7.4.1.2.4 first slice of a new picture? (same tests as the reference, headers.c:1027-1050) */
+	/* 7.4.1.2.4 first slice of a new picture? (same tests as the reference, headers.c:1027-1050, the view included) */
 	if (d->cur >= 0) {
 		const SliceHeader *f = &d->first_sh;
 		int newpic = h->frame_num != f->frame_num || (nal_ref_idc > 0) != (d->cur_nal_ref_idc > 0) || h->idr_pic_id != f->idr_pic_id ||
-		             (s->poc_type == 0 && h->poc_lsb != f->poc_lsb) || (s->poc_type == 1 && h->delta_poc[0] != f->delta_poc[0]);
+		             (s->poc_type == 0 && h->poc_lsb != f->poc_lsb) || (s->poc_type == 1 && h->delta_poc[0] != f->delta_poc[0]) ||
+		             view != d->pics[d->cur].view;
 		if (newpic) { ret = finish_picture(d); if (ret) return ret; }
 	}
-	if (d->cur < 0 && (ret = start_picture(d, h, nal_unit_type == 5, nal_ref_idc))) return ret;
+	d->view = view;
+	if (d->cur < 0 && (ret = start_picture(d, h, idr, nal_ref_idc))) return ret;
 	if (d->cur_skip) return h->first_mb >= d->w_mbs * d->h_mbs ? EBADMSG : 0;   /* its slice data is never parsed */
 	int col_slot;
 	if ((ret = setup_slice(d, p, h, b, *jobp, &col_slot))) return ret;
@@ -1217,7 +1312,8 @@ Edge264Decoder *edge264_alloc(int n_threads, Edge264LogCb log_cb, void *log_arg,
 	Edge264Decoder *d = (Edge264Decoder *)calloc(1, sizeof(*d));
 	if (!d) return NULL;
 	d->alloc_cb = (alloc_cb && free_cb) ? alloc_cb : NULL; d->free_cb = free_cb; d->alloc_arg = alloc_arg;
-	d->cur = -1; d->pending_release = -1; d->prev_ref_frame_num = -1; d->q_prev_ref_frame_num = -1;
+	d->cur = -1; d->base_slot = -1; d->inter_view_flag = 1;
+	for (int v = 0; v < 2; v++) { d->pending_release[v] = -1; d->prev_ref_frame_num[v] = -1; d->q_prev_ref_frame_num[v] = -1; }
 	d->be = e264_default_backend();
 	if (!d->be || d->be->create(&d->be_ctx)) { free(d); return NULL; }
 	d->n_builds = 1;
@@ -1242,9 +1338,11 @@ void edge264_flush(Edge264Decoder *d) {
 	/* drop every picture and the sequence state, keep parameter sets (reference edge264.c:261-270 clears them too) */
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { d->pics[i].in_use = 0; d->pics[i].host_buf = -1; }
 	for (int i = 0; i < E264_MAX_HOSTBUFS; i++) if (d->hb[i].state != 3 || !d->hb[i].borrowed) d->hb[i].state = 0;
-	d->outq_n = 0; d->cur = -1; d->pending_release = -1;
-	d->prev_ref_frame_num = -1; d->q_prev_ref_frame_num = -1; d->prev_ref_poc = 0;
+	d->cur = -1; d->base_slot = -1; d->inter_view_flag = 1;
+	for (int v = 0; v < 2; v++) { d->outq_n[v] = 0; d->pending_release[v] = -1; d->prev_ref_frame_num[v] = -1; d->q_prev_ref_frame_num[v] = -1; d->prev_ref_poc[v] = 0; }
 	memset(&d->sps, 0, sizeof(d->sps)); memset(d->pps, 0, sizeof(d->pps));
+	memset(&d->ssps, 0, sizeof(d->ssps)); d->mvc = 0;   /* stereo off, like the reference's clear_decoder (headers.c:135-141) */
+	memset(d->ref_frame_view, 0, sizeof(d->ref_frame_view));
 	d->configured = 0;
 }
 
@@ -1271,14 +1369,18 @@ int edge264_decode_NAL(Edge264Decoder *d, const uint8_t *buf, const uint8_t *end
 	return r;
 }
 static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t *end, Edge264UnrefCb unref_cb, void *unref_arg) {
-	if (d->pending_release >= 0) { d->hb[d->pending_release].state = 0; d->pending_release = -1; }
+	for (int v = 0; v < 2; v++) if (d->pending_release[v] >= 0) { d->hb[d->pending_release[v]].state = 0; d->pending_release[v] = -1; }
 	if (buf >= end) {
 		int r = bump_all(d);
 		return r ? r : ENODATA;
 	}
 	int nal_ref_idc = buf[0] >> 5, nal_unit_type = buf[0] & 31;
 	size_t n = (size_t)(end - buf) - 1;
-	if (nal_unit_type == 1 || nal_unit_type == 5) {   /* the slice data is parsed from its own copy of the payload, possibly later */
+	if (nal_unit_type == 1 || nal_unit_type == 5 || nal_unit_type == 20) {   /* the slice data is parsed from its own copy of the payload, possibly later */
+		/* NAL unit 20: nal_unit_header_mvc_extension (H.7.3.1.1), then a slice of the second view with the subset SPS and its
+		 * view's DPB (reference headers.c:1309-1332) */
+		const int view = nal_unit_type == 20;
+		if (view && !d->mvc) return EBADMSG;   /* no subset SPS: like a slice without its parameter set */
 		d->slices_seen = 1;
 		SliceJob *job = (SliceJob *)calloc(1, sizeof(SliceJob));
 		/* slack: the slice parsers test for an overrun once per macroblock, so a damaged slice reads past its end */
@@ -1288,7 +1390,14 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 		memset(rb + rn, 0, 32);
 		job->rbsp = rb;
 		BitReader b; br_init(&b, rb, rn);
-		int ret = decode_slice(d, nal_unit_type, nal_ref_idc, &b, &job);
+		int idr = nal_unit_type == 5, ret = 0;
+		if (view) {
+			const uint32_t x = br_u(&b, 24);
+			idr = !(x >> 22 & 1);   /* non_idr_flag */
+			ret = x >> 23 ? ENOTSUP : 0;   /* svc_extension_flag */
+		}
+		if (!(view && ret)) ret = decode_slice(d, nal_unit_type, nal_ref_idc, view, idr, &b, &job);
+		if (!view) d->inter_view_flag = 1;   /* inferred for a base view slice without a prefix NAL unit (H.7.4.1.1) */
 		if (job) { free(rb); free(job); }      /* not queued */
 		if (ret == 0 && unref_cb) unref_cb(0, unref_arg);
 		return ret;
@@ -1300,10 +1409,10 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 	int ret;
 	switch (nal_unit_type) {
 	case 7: {
-		SPS s; ret = parse_sps(d, &b, &s);
+		SPS s; ret = parse_sps(d, &b, &s, 0);
 		if (ret == 0) {
 			int same_format = d->configured && d->sps.width_mbs == s.width_mbs && d->sps.height_mbs == s.height_mbs && !memcmp(d->sps.crop, s.crop, sizeof(s.crop));
-			int fits = same_format && s.max_num_ref_frames + 2 <= d->n_slots;
+			int fits = same_format && s.max_num_ref_frames + 2 + (d->mvc ? d->ssps.max_num_ref_frames : 0) <= d->n_slots;
 			if (!fits) {
 				if (d->configured && bump_all(d)) return ENOBUFS;   /* frame format change: drain first (headers.c:2005-2007) */
 				ret = configure_sequence(d, &s, same_format);
@@ -1313,8 +1422,38 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 			d->sps = s;
 		}
 		break; }
+	case 15: {   /* subset SPS: turns stereo decoding on (edge264_mvc.h) */
+		SPS s; ret = parse_sps(d, &b, &s, 1);
+		if (ret) break;
+		/* the second view has the frame format of its base, and both views' references fit in the 32 frame slots; otherwise
+		 * the stream is decoded as its base view alone */
+		if (!d->configured || d->sps.width_mbs != s.width_mbs || d->sps.height_mbs != s.height_mbs || memcmp(d->sps.crop, s.crop, sizeof(s.crop)) ||
+		    s.max_num_ref_frames > 15 || d->sps.max_num_ref_frames + s.max_num_ref_frames + 2 > E264_MAX_SLOTS) { ret = ENOTSUP; break; }
+		if (!d->mvc || d->sps.max_num_ref_frames + s.max_num_ref_frames + 2 > d->n_slots) {   /* more frame slots: drain first, like a format change */
+			if (bump_all(d)) return ENOBUFS;
+			d->mvc = 1; d->ssps = s;
+			if ((ret = configure_sequence(d, &d->sps, 1))) return ret;
+		}
+		d->ssps = s;
+		break; }
+	case 14: {   /* prefix NAL unit: nal_unit_header_mvc_extension of the base view slice that follows */
+		const uint32_t x = br_u(&b, 24);
+		if (b.overrun) { ret = EBADMSG; break; }
+		if (x >> 23) { ret = ENOTSUP; break; }   /* svc_extension_flag */
+		d->inter_view_flag = x >> 1 & 1;
+		ret = 0;
+		break; }
 	case 8: ret = parse_pps(d, &b); break;
-	case 10: ret = 0; if (d->cur >= 0) finish_picture(d); d->prev_ref_frame_num = -1; break;   /* end of sequence */
+	case 10:   /* end of sequence; a stereo sequence is output in full and the decoder goes back to single view (reference headers.c:143-151) */
+		if (d->mvc) {
+			if (bump_all(d)) return ENOBUFS;
+			const int b = d->base_slot;
+			d->mvc = 0; d->base_slot = -1; memset(&d->ssps, 0, sizeof(d->ssps));
+			for (int v = 0; v < 2; v++) { d->q_prev_ref_frame_num[v] = -1; d->prev_ref_poc[v] = 0; }   /* the reference clears its decoder here */
+			memset(d->ref_frame_view, 0, sizeof(d->ref_frame_view));
+			if (b >= 0) slot_release_if_unused(d, b);
+		}
+		ret = 0; if (d->cur >= 0) finish_picture(d); d->prev_ref_frame_num[0] = d->prev_ref_frame_num[1] = -1; break;
 	case 6: case 9: case 11: case 12: ret = 0; break;
 	default: ret = ENOTSUP;
 	}
@@ -1322,28 +1461,30 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 	return ret;
 }
 
-int edge264_get_frame(Edge264Decoder *d, Edge264Frame *out, int borrow) {
-	if (!d || !out) return EINVAL;
-	if (d->outq_n == 0) return ENOMSG;
-	int hbuf = d->outq[0];
+/* 0: the picture in host buffer hbuf may be output; ENOMSG: not yet; EIO: device error.  Like the reference in threaded mode
+ * (edge264.c:373: a frame whose last macroblock is not deblocked yet answers ENOMSG), a picture still on the device is "not
+ * available yet" — unless the last decode_NAL told the application to fetch frames (ENOBUFS, end of stream): then the call
+ * waits, so that no application loop ever has to poll. */
+static int output_ready(Edge264Decoder *d, int hbuf) {
 	HostBuf *hb = &d->hb[hbuf];
 	if (!__atomic_load_n(&hb->submitted, __ATOMIC_ACQUIRE)) return ENOMSG;   /* queued at insertion but still being parsed */
-	/* Like the reference in threaded mode (edge264.c:373: a frame whose last macroblock is not deblocked yet answers
-	 * ENOMSG), a picture still on the device is "not available yet" — unless the last decode_NAL told the application
-	 * to fetch frames (ENOBUFS, end of stream): then the call waits, so that no application loop ever has to poll. */
 	if (!d->block_output) {
 		int pr = d->be->poll(d->be_ctx, hb->ticket);
 		if (pr == EAGAIN) return ENOMSG;
 		if (pr) return EIO;
 	}
 	{ PROF_BEGIN; int wr = d->be->wait(d->be_ctx, hb->ticket); PROF_END(3); if (wr) return EIO; }
-	memmove(d->outq, d->outq + 1, (size_t)(--d->outq_n) * sizeof(int));
-	*out = d->out_fmt;
-	int top = out->frame_crop_offsets[0], left = out->frame_crop_offsets[3];
-	out->samples[0] = hb->p + top * d->stride_y + left;
-	out->samples[1] = hb->p + d->plane_y + (top >> 1) * d->stride_c + (left >> 1);
-	out->samples[2] = out->samples[1] + (d->stride_c >> 1);
-	out->FrameId = hb->frame_id;
+	return 0;
+}
+/* the samples (cropped) and error map of host buffer hb */
+static void frame_planes(const Edge264Decoder *d, const HostBuf *hb, const Edge264Frame *fmt, const uint8_t *samples[3]) {
+	int top = fmt->frame_crop_offsets[0], left = fmt->frame_crop_offsets[3];
+	samples[0] = hb->p + top * d->stride_y + left;
+	samples[1] = hb->p + d->plane_y + (top >> 1) * d->stride_c + (left >> 1);
+	samples[2] = samples[1] + (d->stride_c >> 1);
+}
+static void frame_map(const Edge264Decoder *d, const HostBuf *hb, Edge264Frame *out) {
+	out->mb_errors = NULL; out->stride_mb = d->out_fmt.stride_mb;
 	/* the map was written for this picture only if some macroblock could be wrong; a map of zeros is reported as none */
 	if (hb->err_pic) {
 		const size_t nmb = (size_t)d->w_mbs * d->h_mbs;
@@ -1351,16 +1492,67 @@ int edge264_get_frame(Edge264Decoder *d, Edge264Frame *out, int borrow) {
 		while (k < nmb && !hb->map[k]) k++;
 		if (k < nmb) { out->mb_errors = hb->map; out->stride_mb = (int16_t)d->w_mbs; }
 	}
-	out->return_arg = (void *)(uintptr_t)(hbuf + 1);
-	hb->state = 3; hb->borrowed = borrow != 0;
-	if (!borrow) d->pending_release = hbuf;   /* valid until the next decode_NAL, as in the reference */
+}
+/* return_arg of an output frame: host buffer + 1 of the base view in bits 0-7, of the second view in bits 8-15 */
+static int frame_hostbuf(const Edge264Frame *f, int view) {
+	const uintptr_t a = (uintptr_t)f->return_arg;
+	return a >> 16 ? -1 : (int)(a >> (8 * view) & 255) - 1;
+}
+
+int edge264_get_frame(Edge264Decoder *d, Edge264Frame *out, int borrow) {
+	if (!d || !out) return EINVAL;
+	/* a stereo sequence outputs a pair once both views of the access unit are ready (reference edge264.c:365-407) */
+	if (d->outq_n[0] == 0 || (d->mvc && d->outq_n[1] == 0)) return ENOMSG;
+	const int pair = d->outq_n[1] > 0, h0 = d->outq[0][0], h1 = pair ? d->outq[1][0] : -1;
+	int r = output_ready(d, h0);
+	if (!r && pair) r = output_ready(d, h1);
+	if (r) return r;
+	*out = d->out_fmt;
+	for (int v = 0; v <= pair; v++) {
+		const int h = v ? h1 : h0;
+		memmove(d->outq[v], d->outq[v] + 1, (size_t)(--d->outq_n[v]) * sizeof(int));
+		d->hb[h].state = 3; d->hb[h].borrowed = borrow != 0;
+		if (!borrow) d->pending_release[v] = h;   /* valid until the next decode_NAL, as in the reference */
+	}
+	frame_planes(d, &d->hb[h0], out, out->samples);
+	out->FrameId = d->hb[h0].frame_id;
+	frame_map(d, &d->hb[h0], out);
+	out->return_arg = (void *)(uintptr_t)(h0 + 1);
+	if (pair) {
+		frame_planes(d, &d->hb[h1], out, out->samples_mvc);
+		out->FrameId_mvc = d->hb[h1].frame_id;
+		out->return_arg = (void *)(uintptr_t)((h0 + 1) | (h1 + 1) << 8);
+	}
 	return 0;
 }
 
 void edge264_return_frame(Edge264Decoder *d, void *return_arg) {
 	if (!d) return;
-	int i = (int)(uintptr_t)return_arg - 1;
-	if (i >= 0 && i < E264_MAX_HOSTBUFS && d->hb[i].state == 3) { d->hb[i].state = 0; d->hb[i].borrowed = 0; if (d->pending_release == i) d->pending_release = -1; }
+	const Edge264Frame f = {.return_arg = return_arg};
+	for (int v = 0; v < 2; v++) {
+		const int i = frame_hostbuf(&f, v);
+		if (i >= 0 && i < E264_MAX_HOSTBUFS && d->hb[i].state == 3) {
+			d->hb[i].state = 0; d->hb[i].borrowed = 0;
+			for (int w = 0; w < 2; w++) if (d->pending_release[w] == i) d->pending_release[w] = -1;
+		}
+	}
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* stereo frames (include/edge264_mvc.h)                                                        */
+/* ------------------------------------------------------------------------------------------ */
+int edge264_get_second_view(Edge264Decoder *d, const Edge264Frame *frame, Edge264Frame *out) {
+	if (!d || !frame || !out) return EINVAL;
+	const int h0 = frame_hostbuf(frame, 0), h1 = frame_hostbuf(frame, 1);
+	if (h0 < 0 || h0 >= E264_MAX_HOSTBUFS || d->hb[h0].state != 3) return EINVAL;
+	if (h1 < 0) return ENOENT;
+	if (h1 >= E264_MAX_HOSTBUFS || d->hb[h1].state != 3) return EINVAL;
+	*out = *frame;
+	for (int p = 0; p < 3; p++) { out->samples[p] = frame->samples_mvc[p]; out->samples_mvc[p] = NULL; }
+	out->FrameId = frame->FrameId_mvc; out->FrameId_mvc = 0;
+	frame_map(d, &d->hb[h1], out);
+	out->return_arg = (void *)(uintptr_t)(h1 + 1);   /* a mono frame of its own for the output getters */
+	return 0;
 }
 
 /* ------------------------------------------------------------------------------------------ */
@@ -1377,7 +1569,7 @@ int edge264_enable_motion(Edge264Decoder *d) {
 int edge264_get_motion(Edge264Decoder *d, const Edge264Frame *frame, Edge264Motion *out) {
 	if (!d || !frame || !out) return EINVAL;
 	if (!d->motion) return ENOENT;
-	const int i = (int)(uintptr_t)frame->return_arg - 1;
+	const int i = frame_hostbuf(frame, 0);
 	if (i < 0 || i >= E264_MAX_HOSTBUFS || d->hb[i].state != 3 || !d->hb[i].motion) return EINVAL;
 	const size_t nmb = (size_t)d->w_mbs * d->h_mbs;
 	const uint8_t *m = d->hb[i].motion;
@@ -1413,7 +1605,7 @@ int edge264_enable_resized(Edge264Decoder *d, int format, int width, int height)
 int edge264_get_packed(Edge264Decoder *d, const Edge264Frame *frame, Edge264Packed *out) {
 	if (!d || !frame || !out) return EINVAL;
 	if (!d->packed) return ENOENT;
-	const int i = (int)(uintptr_t)frame->return_arg - 1;
+	const int i = frame_hostbuf(frame, 0);
 	if (i < 0 || i >= E264_MAX_HOSTBUFS || d->hb[i].state != 3 || !d->hb[i].packed) return EINVAL;
 	const HostBuf *hb = &d->hb[i];
 	const E264PackedLayout l = e264_packed_layout(&hb->pk);
@@ -1439,7 +1631,7 @@ int edge264_enable_picstats(Edge264Decoder *d) {
 int edge264_get_picstats(Edge264Decoder *d, const Edge264Frame *frame, Edge264PicStats *out) {
 	if (!d || !frame || !out) return EINVAL;
 	if (!d->picstats) return ENOENT;
-	const int i = (int)(uintptr_t)frame->return_arg - 1;
+	const int i = frame_hostbuf(frame, 0);
 	if (i < 0 || i >= E264_MAX_HOSTBUFS || d->hb[i].state != 3 || !d->hb[i].picstats) return EINVAL;
 	const size_t nmb = (size_t)d->w_mbs * d->h_mbs;
 	const uint8_t *s = d->hb[i].picstats;

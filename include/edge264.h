@@ -40,7 +40,7 @@ typedef void (*Edge264FreeCb)(void *samples, void *mbs, void *alloc_arg);
 /* One output picture (reference edge264.h:45-62).  Field order and widths are ABI. */
 typedef struct Edge264Frame {
 	const uint8_t *samples[3];      /* Y, Cb, Cr; already offset by the cropping rectangle   */
-	const uint8_t *samples_mvc[3];  /* second view (MVC) — always NULL here                   */
+	const uint8_t *samples_mvc[3];  /* second view of a stereo frame (edge264_mvc.h), else NULL */
 	const uint8_t *mb_errors;       /* NULL when no macroblock can be wrong, else 0..100 per macroblock of the coded
 	                                 * picture, row y at mb_errors + y * stride_mb (= width in macroblocks); pinned
 	                                 * host memory, valid as long as the samples */
@@ -54,7 +54,7 @@ typedef struct Edge264Frame {
 	int16_t stride_C;               /* bytes between two Cb rows (a Cr row sits in between)   */
 	int16_t stride_mb;
 	int32_t FrameId;
-	int32_t FrameId_mvc;
+	int32_t FrameId_mvc;            /* FrameId of the second view, when samples_mvc is set    */
 	int16_t frame_crop_offsets[4];  /* {top,right,bottom,left} in luma samples                */
 	void   *return_arg;             /* pass to edge264_return_frame when borrowed             */
 } Edge264Frame;

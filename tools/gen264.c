@@ -37,6 +37,16 @@
  *          [--cqp-offset A,B]               (chroma_qp_index_offset A and second_chroma_qp_index_offset B in every PPS)
  *          [--levels big]                   (levels up to the 8-bit bound -32768..32767: CAVLC escapes, long CABAC suffixes)
  *          [--pcm-extreme]                  (PCM macroblocks with 0/255 steps, full-range ramps, checkers and random bits)
+ *   stereo (include/edge264_mvc.h):
+ *          [--mvc [seed]]                   (a second view: a subset SPS (Stereo High) after every SPS, a prefix NAL unit before
+ *                                            every base view slice and the second view's slices (NAL unit 20) after the base
+ *                                            view's.  Anchor access units (I or IDR base view) code a P second view predicted
+ *                                            from the base view only; the others a P or B second view whose random reference
+ *                                            choices draw the inter-view reference too.  With --dpb the second view takes list
+ *                                            modifications, idc 4 and 5 included, and memory-management operations.  Base views
+ *                                            with nal_ref_idc 0 carry inter_view_flag 1 or 0, and in the latter case their second
+ *                                            view does not predict from them.  The second view draws from its own generator
+ *                                            seeded by `seed`, so the base view's NAL units are those written without --mvc.)
  */
 #define E264_ENCODER
 #include <stdio.h>
@@ -53,7 +63,15 @@ typedef struct GenPic {
 typedef struct GenState {
 	uint64_t rng;
 	int W, H, frames, cabac, gop, idr_period, refs, t8x8_pct, scaling, wp, slices, deblock, density, qp0, temporal, pcm_pm, crop_bottom, level, mvrange, intra_pct, skip_pct;
-	GenPic dpb[E264_MAX_SLOTS];
+	GenPic *dpb;            /* the pictures of the view being coded: views[0] or, with --mvc, views[1] */
+	GenPic views[2][E264_MAX_SLOTS];
+	int mvc, view;          /* --mvc: a second view is written; the view being coded */
+	uint64_t rng_view;      /* --mvc: the generator of the view not being coded */
+	int max_long_view;      /* --mvc: max_long_idx_plus1 of the view not being coded */
+	const GenPic *base;     /* --mvc: the base view picture of the access unit, the second view's inter-view reference */
+	int base_inter_view;    /* --mvc: inter_view_flag of that base view picture */
+	int au_anchor;          /* the access unit is an anchor (its base view is an I or IDR picture) */
+	GenPic *last_pic;       /* the picture encode_picture coded last */
 	int32_t next_uid;
 	MbInfo *mbi; int16_t *pool;
 	int t8x8_mode;          /* PPS transform_8x8_mode_flag */
@@ -103,9 +121,10 @@ static void put_scaling_matrix(GenState *g, BitWriter *w, int n_lists) {
 	}
 }
 
-static void write_sps(GenState *g, ByteBuf *out) {
+/* subset: the subset SPS of --mvc (NAL unit 15, Stereo High, two views whose second predicts from the first) */
+static void write_sps(GenState *g, ByteBuf *out, int subset) {
 	BitWriter w; bw_init(&w, 4096);
-	bw_u(&w, 8, 100); bw_u(&w, 8, 0); bw_u(&w, 8, g->level);
+	bw_u(&w, 8, subset ? 128 : 100); bw_u(&w, 8, 0); bw_u(&w, 8, g->level);
 	bw_ue(&w, 0);
 	bw_ue(&w, 1); bw_ue(&w, 0); bw_ue(&w, 0); bw_u(&w, 1, 0);
 	bw_u(&w, 1, g->scaling == 1 || g->scaling == 3);
@@ -128,8 +147,22 @@ static void write_sps(GenState *g, ByteBuf *out) {
 	bw_u(&w, 1, 1); bw_ue(&w, 0); bw_ue(&w, 0); bw_ue(&w, 16); bw_ue(&w, 16);
 	bw_ue(&w, g->gop == 2 ? 1 : 0);     /* max_num_reorder_frames */
 	bw_ue(&w, g->refs + (g->gop == 2)); /* max_dec_frame_buffering */
+	if (subset) {
+		bw_u(&w, 1, 1);                      /* bit_equal_to_one */
+		bw_ue(&w, 1); bw_ue(&w, 0); bw_ue(&w, 1);   /* num_views_minus1, view_id 0 and 1 */
+		bw_ue(&w, 1); bw_ue(&w, 0); bw_ue(&w, 0);   /* anchor: l0 holds view 0, l1 nothing */
+		bw_ue(&w, 1); bw_ue(&w, 0); bw_ue(&w, 1); bw_ue(&w, 0);   /* non-anchor: view 0 in l0 and l1 */
+		bw_ue(&w, 0); bw_u(&w, 8, g->level); bw_ue(&w, 0); bw_u(&w, 3, 0); bw_ue(&w, 1); bw_ue(&w, 0); bw_ue(&w, 1); bw_ue(&w, 1);   /* one level, one operation point: both views */
+		bw_u(&w, 1, 0);                      /* mvc_vui_parameters_present_flag */
+		bw_u(&w, 1, 0);                      /* additional_extension2_flag */
+	}
 	bw_trailing(&w);
-	e264_emit_nal(out, 3, 7, w.buf, w.pos / 8); free(w.buf);
+	e264_emit_nal(out, 3, subset ? 15 : 7, w.buf, w.pos / 8); free(w.buf);
+	if (g->mvc && !subset) {   /* its scaling lists are drawn from the second view's generator, which the base view never reads */
+		uint64_t r = g->rng; g->rng = g->rng_view; g->rng_view = r;
+		write_sps(g, out, 1);
+		r = g->rng; g->rng = g->rng_view; g->rng_view = r;
+	}
 }
 static void write_pps(GenState *g, ByteBuf *out, int id, int init_qp) {
 	BitWriter w; bw_init(&w, 4096);
@@ -384,8 +417,13 @@ static void gen_wp_full(GenState *g, int is_b, int n0, int *lwd, int *cwd, int16
 }
 
 /* returns 1 when the picture carried memory_management_control_operation 5 (frame_num and POC restart after it) */
+/* --mvc: the frame slot number the second view's records give the inter-view reference (no picture of its own view uses it) */
+#define IV_SLOT (E264_MAX_SLOTS - 1)
+static const GenPic *gen_pic(const GenState *g, int slot) { return slot == IV_SLOT ? g->base : &g->dpb[slot]; }
+
 static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_pic_id) {
 	int nmb = g->W * g->H;
+	const int anchor = g->au_anchor;   /* --mvc: an anchor access unit, whose second view predicts from the base view only */
 	/* free DPB slot for this picture */
 	int slot = -1;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) if (!g->dpb[i].used) { slot = i; break; }
@@ -396,6 +434,7 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 	cp->frame_num = pp->frame_num; cp->poc = pp->poc; cp->uid = g->next_uid++;
 	if (pp->idr) for (int i = 0; i < E264_MAX_SLOTS; i++) g->dpb[i].used = 0;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) cp->slot_uid[i] = (g->dpb[i].used || i == slot) ? g->dpb[i].uid : -1;
+	if (g->view) cp->slot_uid[IV_SLOT] = g->base->uid;
 
 	/* reference lists exactly as 8.2.4.2 builds them for our simple GOPs (all short-term) */
 	int l0[16], l1[16], n0 = 0, n1 = 0;
@@ -414,11 +453,23 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 			for (int i = 0; i < na; i++) l0[n0++] = af[i];
 			for (int i = 0; i < na; i++) l1[n1++] = af[i];
 			for (int i = 0; i < nb; i++) l1[n1++] = bf[i];
-			if (n1 > 1 && l0[0] == l1[0]) { int t = l1[0]; l1[0] = l1[1]; l1[1] = t; }
 		}
 	}
+	/* the second view's lists end with the inter-view reference (H.8.2.1); an anchor's holds nothing else */
+	const int nt0 = n0, nt1 = n1;
+	if (g->view) { if (anchor) n0 = 0; l0[n0++] = IV_SLOT; if (pp->type == 1) l1[n1++] = IV_SLOT; }
+	if (pp->type == 1 && n1 > 1 && l0[0] == l1[0]) { int t = l1[0]; l1[0] = l1[1]; l1[1] = t; }
 	int num_ref[2] = {n0 < 1 ? 1 : n0, n1 < 1 ? 1 : n1};
-	if (pp->type == 1) { if (num_ref[0] > 2) num_ref[0] = 2; if (num_ref[1] > 2) num_ref[1] = 2; }
+	if (pp->type == 1 && !g->view) { if (num_ref[0] > 2) num_ref[0] = 2; if (num_ref[1] > 2) num_ref[1] = 2; }
+	if (g->view && !g->base_inter_view) { num_ref[0] = nt0; num_ref[1] = nt1; }   /* a base view that is no inter-view reference (B: both lists hold a temporal picture first) */
+	/* --temporal: a P second view is the co-located picture of the B second views after it, and temporal direct needs every
+	 * picture it predicts from in their list 0 (8.4.1.2.3).  Its inter-view reference goes to the front (list modification)
+	 * and it leaves out the picture the sliding window drops when it is marked. */
+	const int iv_front = g->view && !anchor && g->temporal && pp->type == 0;
+	if (iv_front) {
+		for (int i = n0 - 1; i > 0; i--) l0[i] = l0[i - 1];
+		l0[0] = IV_SLOT; num_ref[0] = 1 + (nt0 >= g->refs ? g->refs - 1 : nt0);
+	}
 	g->drift[0] = laplace(g, 6); g->drift[1] = laplace(g, 4);
 	g->cur_is_b = pp->type == 1;
 
@@ -428,7 +479,7 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 	int m_used[E264_MAX_SLOTS], m_long[E264_MAX_SLOTS], m_idx[E264_MAX_SLOTS], m_max = g->max_long_idx_plus1;
 	for (int i = 0; i < E264_MAX_SLOTS; i++) { m_used[i] = g->dpb[i].used && i != slot; m_long[i] = g->dpb[i].is_long; m_idx[i] = g->dpb[i].long_idx; }
 	if (g->dpb_mode && pp->idr) { idr_long = g->refs > 1 && rnd(g, 4) == 0;   /* with one reference frame the reference decoder asserts (edge264_headers.c:1099) */ m_max = idr_long ? 1 : 0; cur_long = idr_long ? 0 : -1; }
-	if (g->dpb_mode && !pp->idr && pp->type == 0 && pp->is_ref) {
+	if (g->dpb_mode && !pp->idr && pp->type == 0 && pp->is_ref && !(g->view && anchor)) {
 		const int maxfn = 1 << g->log2_max_frame_num, cur = pp->frame_num & (maxfn - 1);
 #define DIFF(i) (cur - (((g->dpb[i].frame_num & (maxfn - 1)) > cur) ? (g->dpb[i].frame_num & (maxfn - 1)) - maxfn : (g->dpb[i].frame_num & (maxfn - 1))))
 #define PICK(cond, out) do { int c_[E264_MAX_SLOTS], n_ = 0; for (int i = 0; i < E264_MAX_SLOTS; i++) if (m_used[i] && (cond)) c_[n_++] = i; out = n_ ? c_[rnd(g, n_)] : -1; } while (0)
@@ -470,6 +521,10 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 		int last_mb = (sl + 1) * rows_per_slice * g->W; if (last_mb > nmb) last_mb = nmb;
 		int pps_id = st == 2 ? 0 : st == 0 ? 1 : 2;
 		BitWriter w; bw_init(&w, 1 << 16);
+		/* nal_unit_header_mvc_extension: non_idr_flag, priority_id 0, view_id, temporal_id 0, anchor_pic_flag, inter_view_flag
+		 * (the second view is no one's reference), reserved_one_bit */
+		const uint32_t mvc_hdr = (uint32_t)!pp->idr << 22 | (uint32_t)g->view << 6 | (uint32_t)anchor << 2 | (uint32_t)(!g->view && g->base_inter_view) << 1 | 1;
+		if (g->view) bw_u(&w, 24, mvc_hdr);
 		bw_ue(&w, first_mb);
 		bw_ue(&w, st + (rnd(g, 2) ? 5 : 0));
 		bw_ue(&w, pps_id);
@@ -482,12 +537,20 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 			bw_u(&w, 1, 1);   /* num_ref_idx_active_override_flag */
 			bw_ue(&w, num_ref[0] - 1);
 			if (st == 1) bw_ue(&w, num_ref[1] - 1);
-			if (g->dpb_mode && st == 0 && n0 > 0 && rnd(g, 2)) {   /* ref_pic_list_modification (7.3.3.1, 8.2.4.3): move existing pictures to the front */
+			if ((g->view && anchor && !pp->idr) || iv_front) {   /* the inter-view reference to the front: a non-IDR anchor uses it alone */
+				bw_u(&w, 1, 1); bw_ue(&w, 5); bw_ue(&w, 0); bw_ue(&w, 3);
+			} else if (g->dpb_mode && st == 0 && n0 > 0 && rnd(g, 2)) {   /* ref_pic_list_modification (7.3.3.1, 8.2.4.3): move existing pictures to the front */
 				bw_u(&w, 1, 1); g->stat_rplm++;
 				const int maxfn = 1 << g->log2_max_frame_num;
-				int pred = pp->frame_num & (maxfn - 1), nops = 1 + rnd(g, num_ref[0] < 3 ? num_ref[0] : 3);
+				int pred = pp->frame_num & (maxfn - 1), nops = 1 + rnd(g, num_ref[0] < 3 ? num_ref[0] : 3), view_pred = -1;
 				for (int k = 0; k < nops; k++) {
-					const GenPic *t = &g->dpb[l0[rnd(g, n0)]];
+					const int ti = l0[rnd(g, n0)];
+					if (ti == IV_SLOT) {   /* H.8.2.2.3: idc 5 adds abs_diff_view_idx_minus1 + 1 to the view index prediction (-1 first), idc 4 subtracts it, modulo the one inter-view reference */
+						if (!g->base_inter_view) continue;
+						bw_ue(&w, view_pred < 0 ? 5 : 4); bw_ue(&w, 0); view_pred = 0;
+						continue;
+					}
+					const GenPic *t = &g->dpb[ti];
 					if (t->is_long) { bw_ue(&w, 2); bw_ue(&w, t->long_idx); continue; }
 					const int nowrap = t->frame_num & (maxfn - 1);   /* picNumL0NoWrap of a frame is its frame_num */
 					if (nowrap == pred) continue;
@@ -554,7 +617,7 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 		int pic_init_qp = g->qp0;
 		bw_se(&w, slice_qp - pic_init_qp);
 		int idc = g->deblock;
-		const int off = g->deblock_off == 2 || (g->deblock_off == 1 && !pp->is_ref);
+		const int off = g->deblock_off == 2 || (g->deblock_off == 1 && !pp->is_ref && !(g->mvc && !g->view && g->base_inter_view));   /* an inter-view reference counts as a reference (edge264_mvc.h) */
 		bw_ue(&w, off ? 1 : idc);
 		if (idc != 1) {   /* the offsets are drawn either way, so that the rest of the stream does not change */
 			const int a = rnd(g, 13) - 6, b = rnd(g, 13) - 6;
@@ -572,9 +635,9 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 		s->qp = slice_qp; s->deblock_idc = idc; s->cur_poc = pp->poc;
 		s->mbi = g->mbi; s->recs = cp->recs; s->coefs = g->pool; s->coef_cap = (uint32_t)nmb * 408; s->n_coefs = 0;
 		memset(s->ref_slot, -1, sizeof(s->ref_slot));
-		for (int i = 0; i < n0 && i < 16; i++) { s->ref_slot[0][i] = (int8_t)l0[i]; s->ref_uid[0][i] = g->dpb[l0[i]].uid; s->ref_poc[0][i] = g->dpb[l0[i]].poc; }
-		for (int i = 0; i < n1 && i < 16; i++) { s->ref_slot[1][i] = (int8_t)l1[i]; s->ref_uid[1][i] = g->dpb[l1[i]].uid; s->ref_poc[1][i] = g->dpb[l1[i]].poc; }
-		if (st == 1 && n1 > 0) { s->col_recs = g->dpb[l1[0]].recs; s->col_slot_uid = g->dpb[l1[0]].slot_uid; }
+		for (int i = 0; i < n0 && i < 16; i++) { s->ref_slot[0][i] = (int8_t)l0[i]; s->ref_uid[0][i] = gen_pic(g, l0[i])->uid; s->ref_poc[0][i] = gen_pic(g, l0[i])->poc; }
+		for (int i = 0; i < n1 && i < 16; i++) { s->ref_slot[1][i] = (int8_t)l1[i]; s->ref_uid[1][i] = gen_pic(g, l1[i])->uid; s->ref_poc[1][i] = gen_pic(g, l1[i])->poc; }
+		if (st == 1 && n1 > 0) { s->col_recs = gen_pic(g, l1[0])->recs; s->col_slot_uid = gen_pic(g, l1[0])->slot_uid; }
 		s->skip_run = 0;
 		if (g->cabac) {
 			while (w.pos & 7) bw_u(&w, 1, 1);   /* cabac_alignment_one_bit */
@@ -592,12 +655,17 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 		}
 		if (g->cabac) bw_align_zero(&w);   /* the arithmetic coder's last bit is the rbsp_stop_one_bit */
 		else { if (s->skip_run > 0) bw_ue(&w, s->skip_run); bw_trailing(&w); }
-		e264_emit_nal(out, pp->is_ref ? 2 + pp->idr : 0, pp->idr ? 5 : 1, w.buf, w.pos / 8);
+		if (g->mvc && !g->view) {   /* prefix NAL unit of the base view slice: its nal_unit_header_mvc_extension alone */
+			const uint8_t prefix[3] = {(uint8_t)(mvc_hdr >> 16), (uint8_t)(mvc_hdr >> 8), (uint8_t)mvc_hdr};
+			e264_emit_nal(out, pp->is_ref ? 2 + pp->idr : 0, 14, prefix, 3);
+		}
+		e264_emit_nal(out, pp->is_ref ? 2 + pp->idr : 0, g->view ? 20 : pp->idr ? 5 : 1, w.buf, w.pos / 8);
 		free(w.buf); free(s);
 	}
 	for (int k = 0; k < n_mmco; k++) g->stat_mmco[mmco[k][0]]++;
 	if (getenv("GEN264_DEBUG")) { fprintf(stderr, "pic uid %d type %d idr %d frame_num %d poc %d refs %d:", cp->uid, pp->type, pp->idr, pp->frame_num, pp->poc, n0); for (int k = 0; k < n_mmco; k++) fprintf(stderr, " mmco%d(%d,%d)", mmco[k][0], mmco[k][1], mmco[k][2]); fprintf(stderr, "%s\n", idr_long ? " long-term IDR" : ""); }
 	g->stat_idr_long += idr_long;
+	g->last_pic = cp;
 	/* marking: the planned memory-management operations, or the sliding window (8.2.5.3) */
 	if (pp->is_ref) {
 		if (n_mmco || (g->dpb_mode && pp->idr)) {
@@ -617,6 +685,31 @@ static int encode_picture(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_
 		}
 	}
 	return did_op5;
+}
+
+/* --mvc: the coding state of the other view (its pictures, generator and long-term index bound) becomes the current one */
+static void switch_view(GenState *g) {
+	uint64_t r = g->rng; g->rng = g->rng_view; g->rng_view = r;
+	int m = g->max_long_idx_plus1; g->max_long_idx_plus1 = g->max_long_view; g->max_long_view = m;
+	g->view ^= 1; g->dpb = g->views[g->view];
+}
+
+/* one access unit: its base view picture, then with --mvc its second view (same type, frame_num, POC and nal_ref_idc; an I
+ * base view gets a P second view).  Returns encode_picture's result for the base view. */
+static int encode_au(GenState *g, ByteBuf *out, const PicPlan *pp, int idr_pic_id) {
+	g->au_anchor = pp->idr || pp->type == 2;
+	if (!g->mvc) return encode_picture(g, out, pp, idr_pic_id);
+	switch_view(g);
+	g->base_inter_view = pp->is_ref || rnd(g, 2);   /* a non-reference base view may still be an inter-view reference */
+	switch_view(g);
+	const int r = encode_picture(g, out, pp, idr_pic_id);
+	g->base = g->last_pic;
+	switch_view(g);
+	PicPlan q = *pp;
+	if (q.type == 2) q.type = 0;
+	encode_picture(g, out, &q, idr_pic_id);
+	switch_view(g);
+	return r;
 }
 
 static int argi(int argc, char **argv, const char *name, int def) {
@@ -668,6 +761,15 @@ int main(int argc, char **argv) {
 		if (!strcmp(argv[i], "--cqp-offset")) g->cqp_fixed = sscanf(argv[i + 1], "%d,%d", &g->cqp[0], &g->cqp[1]) == 2;
 	}
 	g->qp_walk = argf(argc, argv, "--qp-walk"); g->pcm_extreme = argf(argc, argv, "--pcm-extreme");
+	g->dpb = g->views[0];
+	for (int i = 1; i < argc; i++) if (!strcmp(argv[i], "--mvc")) {
+		g->mvc = 1;
+		const uint64_t seed = i + 1 < argc && argv[i + 1][0] >= '0' && argv[i + 1][0] <= '9' ? strtoull(argv[i + 1], NULL, 10) : 1;
+		g->rng_view = 0x6A09E667F3BCC909ull ^ (seed * 0xD1B54A32D192ED03ull);
+	}
+	/* --mmco5, and --bref or --dpb beside --temporal, would make second views whose co-located pictures predict from
+	 * pictures no longer in the list 0 of the B pictures after them (8.4.1.2.3) */
+	if (g->mvc && (g->mmco5 || (g->temporal && (g->bref || g->dpb_mode)))) { fprintf(stderr, "gen264: --mvc does not combine with --mmco5, nor --temporal with --bref or --dpb\n"); return 2; }
 	if (g->cqp_fixed && (g->cqp[0] < -12 || g->cqp[0] > 12 || g->cqp[1] < -12 || g->cqp[1] > 12)) { fprintf(stderr, "gen264: --cqp-offset takes two offsets in -12..12\n"); return 2; }
 	if ((g->dpb_mode && g->gop == 0) || (g->poc_type && g->gop != 1)) { fprintf(stderr, "gen264: --dpb needs --gop IP or IPB, --poc-type needs --gop IP\n"); return 2; }
 	if (g->slices > g->H) g->slices = g->H;
@@ -683,15 +785,15 @@ int main(int argc, char **argv) {
 	for (int k = 0; k < g->frames;) {
 		int need_idr = k == 0 || since_idr >= g->idr_period;
 		if (g->gop == 0 || need_idr) {
-			write_sps(g, &out);
+			write_sps(g, &out, 0);
 			for (int id = 0; id < 3; id++) write_pps(g, &out, id, g->qp0);
 			PicPlan p = {2, 1, 1, 0, 0};
 			frame_num = 0; disp = 0; since_idr = 0;
-			encode_picture(g, &out, &p, idr_id++ & 0xffff);
+			encode_au(g, &out, &p, idr_id++ & 0xffff);
 			frame_num = 1; disp = 1; since_idr = 1; since_i = 1; k++;
 			continue;
 		}
-		if (g->ps_update && rnd(g, 4) == 0) { if (rnd(g, 3) == 0) write_sps(g, &out); for (int id = 0; id < 3; id++) write_pps(g, &out, id, g->qp0); }
+		if (g->ps_update && rnd(g, 4) == 0) { if (rnd(g, 3) == 0) write_sps(g, &out, 0); for (int id = 0; id < 3; id++) write_pps(g, &out, id, g->qp0); }
 		if (g->extra_nals) {
 			if (rnd(g, 2)) { uint8_t aud[1] = {(uint8_t)(rnd(g, 3) << 5 | 0x10)}; e264_emit_nal(&out, 0, 9, aud, 1); }
 			if (rnd(g, 3) == 0) { uint8_t sei[40]; int n = 2 + rnd(g, 30); sei[0] = 5; sei[1] = (uint8_t)n; for (int i = 0; i < n; i++) sei[2 + i] = (uint8_t)rnd(g, 256); sei[2 + n] = 0x80; e264_emit_nal(&out, 0, 6, sei, 3 + n); }
@@ -702,7 +804,7 @@ int main(int argc, char **argv) {
 		if (g->gop == 1) {
 			const int is_ref = i_pic || !(g->nonref_p && g->poc_type == 0 && !g->dpb_mode && rnd(g, 3) == 0);
 			PicPlan p = {i_pic ? 2 : 0, 0, is_ref, frame_num, disp * 2};
-			if (encode_picture(g, &out, &p, 0)) { frame_num = 0; disp = 0; }
+			if (encode_au(g, &out, &p, 0)) { frame_num = 0; disp = 0; }
 			if (is_ref) frame_num++;
 			disp++; since_idr++; since_i++; k++;
 			continue;
@@ -712,13 +814,13 @@ int main(int argc, char **argv) {
 		if (k + 1 + nb > g->frames) nb = g->frames - k - 1;
 		if (since_idr + 1 + nb > g->idr_period) nb = g->idr_period - since_idr - 1 < 0 ? 0 : g->idr_period - since_idr - 1;
 		PicPlan p = {i_pic ? 2 : 0, 0, 1, frame_num, (disp + nb) * 2};
-		encode_picture(g, &out, &p, 0);
+		encode_au(g, &out, &p, 0);
 		frame_num++; k++;
 		for (int b = 0; b < nb; b++) {
 			int used = 0, nshort = 0;
 			for (int i = 0; i < E264_MAX_SLOTS; i++) if (g->dpb[i].used) { used++; nshort += !g->dpb[i].is_long; }
 			const int can_ref = used < g->refs || nshort > 0;   /* the sliding window needs a short-term picture to drop */
-			PicPlan q = {1, 0, g->bref && b == 0 && nb == 2 && can_ref, frame_num, (disp + b) * 2}; encode_picture(g, &out, &q, 0); if (q.is_ref) frame_num++; k++;
+			PicPlan q = {1, 0, g->bref && b == 0 && nb == 2 && can_ref, frame_num, (disp + b) * 2}; encode_au(g, &out, &q, 0); if (q.is_ref) frame_num++; k++;
 		}
 		disp += nb + 1; since_idr += nb + 1; since_i += nb + 1;
 	}
