@@ -10,7 +10,7 @@ all: $(LIB) tools/gen264 tools/b200_decode tools/libe264bench.so oracle
 
 $(CSRC)/recon.o: $(CSRC)/recon.cu $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/e264b_recon.h
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c $< -o $@ 2> $(CSRC)/recon.ptxas.log || (cat $(CSRC)/recon.ptxas.log; false)
-$(CSRC)/decoder.o: $(CSRC)/decoder.c $(wildcard $(CSRC)/*.h) include/edge264_motion.h include/edge264_packed.h include/edge264_skip.h include/edge264_luma.h include/edge264_picstats.h include/edge264_loopfilter.h include/edge264_mvc.h
+$(CSRC)/decoder.o: $(CSRC)/decoder.c $(wildcard $(CSRC)/*.h) include/edge264_motion.h include/edge264_packed.h include/edge264_skip.h include/edge264_luma.h include/edge264_picstats.h include/edge264_loopfilter.h include/edge264_mvc.h include/edge264_latency.h
 	$(CC) $(CFLAGS) -c $< -o $@
 $(CSRC)/slice_dec.o: $(CSRC)/slice_dec.c $(wildcard $(CSRC)/*.h)
 	$(CC) $(CFLAGS) -c $< -o $@

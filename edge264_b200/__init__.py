@@ -93,6 +93,8 @@ def bind(path):
         lib.edge264_get_picstats.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264PicStats)]
     if hasattr(lib, "edge264_get_second_view"):   # the extension of include/edge264_mvc.h
         lib.edge264_get_second_view.argtypes = [ctypes.c_void_p, ctypes.POINTER(Edge264Frame), ctypes.POINTER(Edge264Frame)]
+    if hasattr(lib, "edge264_set_output_latency"):   # the extension of include/edge264_latency.h
+        lib.edge264_set_output_latency.argtypes = [ctypes.c_void_p, ctypes.c_int]
     _loaded[path] = lib
     return lib
 
@@ -207,7 +209,7 @@ def frame_second_view(lib, dec, f):
 
 
 def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed=None, skip=SKIP_NONE, resized=None, luma_only=False, picstats=False, loop_filter=LOOP_FILTER_ALL,
-                 second_view=False):
+                 second_view=False, output_latency=-1):
     """Decode an Annex-B byte string with the README loop (reference README.md:117-156).
     Returns (frames, return_codes) where frames = [(FrameId, width, height, i420_bytes), ...]; with errors=True each
     frame tuple also carries its per-macroblock error map (bytes, 0..100 per macroblock) or None; with motion=True it
@@ -219,7 +221,9 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
     the non-reference / all pictures without deblocking (edge264_set_loop_filter); second_view=True appends the second
     view of a stereo frame (include/edge264_mvc.h), None for a single-view frame, else a tuple laid out like the frame
     tuple itself (FrameId_mvc, width, height, i420_bytes and the same optional elements).  A library without
-    edge264_get_second_view (the reference's) gives the second view's FrameId, size and samples only."""
+    edge264_get_second_view (the reference's) gives the second view's FrameId, size and samples only.  output_latency=N
+    (0..16) caps the output reorder depth at N and waits for each due frame the device is finishing
+    (edge264_set_output_latency)."""
     gpu = lib is None
     if gpu:
         lib = load()
@@ -264,6 +268,12 @@ def decode_bytes(data, lib=None, n_threads=0, errors=False, motion=False, packed
             d = ctypes.c_void_p(dec)
             lib.edge264_free(ctypes.byref(d))
             raise RuntimeError("edge264_set_loop_filter: %s" % errno.errorcode.get(r, r))
+    if output_latency != -1:
+        r = lib.edge264_set_output_latency(dec, output_latency) if hasattr(lib, "edge264_set_output_latency") else errno.ENOTSUP
+        if r:
+            d = ctypes.c_void_p(dec)
+            lib.edge264_free(ctypes.byref(d))
+            raise RuntimeError("edge264_set_output_latency: %s" % errno.errorcode.get(r, r))
     if picstats:
         r = lib.edge264_enable_picstats(dec) if hasattr(lib, "edge264_enable_picstats") else errno.ENOTSUP
         if r:

@@ -170,6 +170,8 @@ typedef struct PicBuild {
 	int32_t slot_ids[E264_MAX_SLOTS];   /* FrameId held by every frame slot when the picture started (Pic.slot_uid): the motion export's table */
 	uint32_t ref_mask;        /* frame slots the picture's records may predict from */
 	int in_use, closed, running, parsed;
+	int close_complete;       /* a worker closes the picture once its slices cover every macroblock (edge264_latency.h) */
+	int held;                 /* the calling thread is adding a slice: no worker may close the picture meanwhile */
 	uint64_t seq;
 	E264PicDesc pd;           /* filled when parsed: what goes to the backend when the picture's turn comes */
 	SliceJob *head, *tail;
@@ -233,6 +235,8 @@ struct Edge264Decoder {
 	int cur_skip;                      /* the current picture is skipped: its headers run, its slice data is dropped */
 	int skip_mode;                     /* edge264_set_skip: applied to each picture at its first slice */
 	int loop_filter_mode;              /* edge264_set_loop_filter: applied to each picture at its first slice */
+	int output_latency;                /* edge264_set_output_latency: -1, or the cap on the reorder depth, applied to each picture at its first slice */
+	int low_latency;                   /* output_latency >= 0 at the last picture's first slice: get_frame waits for closed pictures */
 	int prev_ref_frame_num[2], prev_ref_poc[2];   /* per view: frame_num and POC of the previous reference picture (8.2.1) */
 	int q_prev_ref_frame_num[2], q_cur_frame_num;   /* reference-style absolute frame numbers, only used to number FrameIds like it */
 	int32_t next_uid;

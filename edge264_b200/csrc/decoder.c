@@ -22,6 +22,7 @@
 #include "../../include/edge264_luma.h"
 #include "../../include/edge264_loopfilter.h"
 #include "../../include/edge264_mvc.h"
+#include "../../include/edge264_latency.h"
 
 /* optional host-side time accounting (E264_HOST_PROFILE=1): where decode_NAL/get_frame spend their time */
 #include <time.h>
@@ -506,10 +507,12 @@ static int finish_picture(Edge264Decoder *d) {
 	d->view = p->view;
 	if (d->pb) {   /* a skipped picture has no build */
 		pthread_mutex_lock(&d->lock);
-		d->pb->conceal_ref = conceal_reference(d);
-		d->pb->closed = 1;
-		pthread_cond_broadcast(&d->work_cv);
-		if (!d->n_threads) ret = build_work(d, d->pb);
+		if (!d->pb->closed) {   /* a worker closes a complete picture itself in low-latency output (build_work) */
+			d->pb->conceal_ref = conceal_reference(d);
+			d->pb->closed = 1;
+			pthread_cond_broadcast(&d->work_cv);
+			if (!d->n_threads) ret = build_work(d, d->pb);
+		}
 		pthread_mutex_unlock(&d->lock);
 		d->pb = NULL;
 	}
@@ -560,6 +563,7 @@ static void slice_enqueue(Edge264Decoder *d, PicBuild *pb, SliceJob *job, int co
 	}
 	if (pb->tail) pb->tail->next = job; else pb->head = job;
 	pb->tail = job;
+	pb->held = 0;
 	pthread_cond_broadcast(&d->work_cv);
 	pthread_mutex_unlock(&d->lock);
 }
@@ -598,6 +602,9 @@ static int build_work(Edge264Decoder *d, PicBuild *pb) {
 		if (job->col_slot >= 0) { d->slot_users[job->col_slot]--; pthread_cond_broadcast(&d->done_cv); }
 		free(job);
 	}
+	/* low-latency output with workers (edge264_latency.h): the picture is closed as soon as its slices cover every
+	 * macroblock, like the synchronous path does in decode_slice, instead of by the next picture's first slice */
+	if (!pb->head && !pb->closed && pb->close_complete && !pb->held && pb->mbs_done >= d->w_mbs * d->h_mbs) pb->closed = 1;
 	if (!pb->head && pb->closed) {
 		pthread_mutex_unlock(&d->lock);
 		build_finalize(d, pb, &pb->pd);
@@ -1107,6 +1114,9 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 	int hbuf = -1;
 	if (!skip && (hbuf = hostbuf_acquire(d)) < 0) return ENOBUFS;
 	if (!v) d->au_skip = skip;
+	/* edge264_latency.h: read at the picture's first slice, like the skip and loop filter modes */
+	const int max_reorder = d->output_latency >= 0 && d->output_latency < s->max_num_reorder_frames ? d->output_latency : s->max_num_reorder_frames;
+	d->low_latency = d->output_latency >= 0;
 	/* absolute (unwrapped) frame numbers like the reference (headers.c:1059) */
 	int prev = d->prev_ref_frame_num[v];
 	int frame_num_abs = idr ? 0 : prev + 1 + ((h->frame_num - prev - 1) & ((1 << s->log2_max_frame_num) - 1));
@@ -1136,6 +1146,7 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 		/* edge264_loopfilter.h: decided once, at the picture's first slice, like the skip decision; for each view component,
 		 * a base view with inter_view_flag counting as a reference */
 		d->pb->no_deblock = d->loop_filter_mode == EDGE264_LOOP_FILTER_NONE || (d->loop_filter_mode == EDGE264_LOOP_FILTER_REF && !(v ? nal_ref_idc : reference));
+		d->pb->close_complete = d->low_latency && d->n_threads;
 	}
 
 	/* IDR / MMCO5: every earlier picture leaves in output order first (reference headers.c:632, 680) */
@@ -1145,7 +1156,8 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 		while (bump_frame(d, v, slot));
 		if (has_mmco5) { cp->poc_top -= cp->poc; cp->poc = 0; }   /* tempPicOrderCnt subtraction (8.2.1) for output order and later pictures; frame_num restarts in apply_marking, once the picture's own lists and operations have used the real value */
 	}
-	/* C.4.5.3 bumping before insertion (reference headers.c:1229-1250) */
+	/* C.4.5.3 bumping before insertion (reference headers.c:1229-1250), with max_num_reorder_frames capped by
+	 * edge264_set_output_latency: the bumping of a stream whose VUI states that depth */
 	int max_bump = s->max_num_ref_frames;
 	if (!nal_ref_idc) {
 		max_bump = 0;
@@ -1156,7 +1168,7 @@ static int start_picture(Edge264Decoder *d, const SliceHeader *h, int idr, int n
 	if (max_bump < 0) {   /* nothing may precede it: straight to the output queue (it is returned once decoded) */
 		cp->needed_for_output = 0;
 		if (!skip) { d->hb[hbuf].state = 2; d->outq[v][d->outq_n[v]++] = hbuf; }
-	} else if (waiting_for_output(d) - !counted > s->max_num_reorder_frames) bump_frame(d, v, -1);
+	} else if (waiting_for_output(d) - !counted > max_reorder) bump_frame(d, v, -1);
 	/* POC bookkeeping for the next picture (8.2.1.1) */
 	if (nal_ref_idc) { d->prev_ref_poc[v] = has_mmco5 ? cp->poc_top : poc_top; }
 	if (has_mmco5) d->prev_ref_frame_num[v] = 0;
@@ -1266,6 +1278,26 @@ static int setup_slice(Edge264Decoder *d, const PPS *p, const SliceHeader *h, co
 	return 0;
 }
 
+/* Low-latency output with workers: a slice that continues the current picture may arrive after a worker has closed it
+ * (its slices already covered every macroblock).  build_hold returns 1 when that happened: the slice then starts a new
+ * picture, as it does without workers.  Otherwise the picture stays open until the slice is queued (slice_enqueue) or
+ * dropped (build_release, which closes the picture if it became complete meanwhile). */
+static int build_hold(Edge264Decoder *d) {
+	pthread_mutex_lock(&d->lock);
+	const int closed = d->pb->closed;
+	d->pb->held = !closed;
+	pthread_mutex_unlock(&d->lock);
+	return closed;
+}
+static void build_release(Edge264Decoder *d) {
+	PicBuild *pb = d->pb;
+	if (!pb || !pb->held) return;
+	pthread_mutex_lock(&d->lock);
+	pb->held = 0;
+	if (!pb->head && !pb->running && pb->mbs_done >= d->w_mbs * d->h_mbs) { pb->closed = 1; pthread_cond_broadcast(&d->work_cv); }
+	pthread_mutex_unlock(&d->lock);
+}
+
 /* Parses the slice header, starts a picture when it is the first slice of one and queues the slice's data on the
  * picture's build.  *jobp is set to NULL once the job is queued; until then it stays the caller's. */
 static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, int view, int idr, BitReader *b, SliceJob **jobp) {
@@ -1282,13 +1314,14 @@ static int decode_slice(Edge264Decoder *d, int nal_unit_type, int nal_ref_idc, i
 		int newpic = h->frame_num != f->frame_num || (nal_ref_idc > 0) != (d->cur_nal_ref_idc > 0) || h->idr_pic_id != f->idr_pic_id ||
 		             (s->poc_type == 0 && h->poc_lsb != f->poc_lsb) || (s->poc_type == 1 && h->delta_poc[0] != f->delta_poc[0]) ||
 		             view != d->pics[d->cur].view;
+		if (!newpic && d->pb && d->pb->close_complete) newpic = build_hold(d);
 		if (newpic) { ret = finish_picture(d); if (ret) return ret; }
 	}
 	d->view = view;
 	if (d->cur < 0 && (ret = start_picture(d, h, idr, nal_ref_idc))) return ret;
 	if (d->cur_skip) return h->first_mb >= d->w_mbs * d->h_mbs ? EBADMSG : 0;   /* its slice data is never parsed */
 	int col_slot;
-	if ((ret = setup_slice(d, p, h, b, *jobp, &col_slot))) return ret;
+	if ((ret = setup_slice(d, p, h, b, *jobp, &col_slot))) { build_release(d); return ret; }
 	PicBuild *pb = d->pb;
 	slice_enqueue(d, pb, *jobp, col_slot);
 	*jobp = NULL;
@@ -1312,7 +1345,7 @@ Edge264Decoder *edge264_alloc(int n_threads, Edge264LogCb log_cb, void *log_arg,
 	Edge264Decoder *d = (Edge264Decoder *)calloc(1, sizeof(*d));
 	if (!d) return NULL;
 	d->alloc_cb = (alloc_cb && free_cb) ? alloc_cb : NULL; d->free_cb = free_cb; d->alloc_arg = alloc_arg;
-	d->cur = -1; d->base_slot = -1; d->inter_view_flag = 1;
+	d->cur = -1; d->base_slot = -1; d->inter_view_flag = 1; d->output_latency = -1;
 	for (int v = 0; v < 2; v++) { d->pending_release[v] = -1; d->prev_ref_frame_num[v] = -1; d->q_prev_ref_frame_num[v] = -1; }
 	d->be = e264_default_backend();
 	if (!d->be || d->be->create(&d->be_ctx)) { free(d); return NULL; }
@@ -1461,14 +1494,30 @@ static int decode_NAL_inner(Edge264Decoder *d, const uint8_t *buf, const uint8_t
 	return ret;
 }
 
+/* Low-latency output: waits until the picture in host buffer hbuf has been handed to the backend if it is closed, that is
+ * if no slice can join it any more and only workers still parse it.  Returns whether it has been handed over; an open
+ * picture is never waited for, since its next slices have not been passed in yet. */
+static int wait_submitted(Edge264Decoder *d, int hbuf) {
+	pthread_mutex_lock(&d->lock);
+	for (;;) {
+		if (__atomic_load_n(&d->hb[hbuf].submitted, __ATOMIC_ACQUIRE)) break;
+		const PicBuild *pb = NULL;
+		for (int i = 0; i < d->n_builds; i++) if (d->builds[i].in_use && d->builds[i].host_buf == hbuf) pb = &d->builds[i];
+		if (!pb || !pb->closed) break;
+		pthread_cond_wait(&d->done_cv, &d->lock);   /* not reached without workers: closing a picture submits it */
+	}
+	pthread_mutex_unlock(&d->lock);
+	return __atomic_load_n(&d->hb[hbuf].submitted, __ATOMIC_ACQUIRE);
+}
 /* 0: the picture in host buffer hbuf may be output; ENOMSG: not yet; EIO: device error.  Like the reference in threaded mode
  * (edge264.c:373: a frame whose last macroblock is not deblocked yet answers ENOMSG), a picture still on the device is "not
- * available yet" — unless the last decode_NAL told the application to fetch frames (ENOBUFS, end of stream): then the call
- * waits, so that no application loop ever has to poll. */
+ * available yet" — unless the last decode_NAL told the application to fetch frames (ENOBUFS, end of stream) or the decoder
+ * is in low-latency output (edge264_latency.h): then the call waits, so that no application loop ever has to poll. */
 static int output_ready(Edge264Decoder *d, int hbuf) {
 	HostBuf *hb = &d->hb[hbuf];
-	if (!__atomic_load_n(&hb->submitted, __ATOMIC_ACQUIRE)) return ENOMSG;   /* queued at insertion but still being parsed */
-	if (!d->block_output) {
+	/* queued at insertion but still being parsed */
+	if (!__atomic_load_n(&hb->submitted, __ATOMIC_ACQUIRE) && !(d->low_latency && wait_submitted(d, hbuf))) return ENOMSG;
+	if (!d->block_output && !d->low_latency) {
 		int pr = d->be->poll(d->be_ctx, hb->ticket);
 		if (pr == EAGAIN) return ENOMSG;
 		if (pr) return EIO;
@@ -1673,5 +1722,14 @@ int edge264_enable_luma_only(Edge264Decoder *d) {
 int edge264_set_loop_filter(Edge264Decoder *d, int mode) {
 	if (!d || mode < EDGE264_LOOP_FILTER_ALL || mode > EDGE264_LOOP_FILTER_NONE) return EINVAL;
 	d->loop_filter_mode = mode;   /* read by start_picture only: the current picture keeps its decision */
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* low-latency output (include/edge264_latency.h)                                               */
+/* ------------------------------------------------------------------------------------------ */
+int edge264_set_output_latency(Edge264Decoder *d, int max_reorder) {
+	if (!d || max_reorder < -1 || max_reorder > 16) return EINVAL;
+	d->output_latency = max_reorder;   /* read by start_picture only: the current picture keeps its depth */
 	return 0;
 }

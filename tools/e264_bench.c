@@ -12,9 +12,11 @@
 #include <time.h>
 #include "edge264.h"
 
-/* include/edge264_luma.h and include/edge264_loopfilter.h; weak: the reference's library has no such entry points */
+/* include/edge264_luma.h, include/edge264_loopfilter.h and include/edge264_latency.h; weak: the reference's library has no
+ * such entry points */
 int edge264_enable_luma_only(Edge264Decoder *dec) __attribute__((weak));
 int edge264_set_loop_filter(Edge264Decoder *dec, int mode) __attribute__((weak));
+int edge264_set_output_latency(Edge264Decoder *dec, int max_reorder) __attribute__((weak));
 
 typedef struct Job {
 	const uint8_t *buf; size_t size;
@@ -53,6 +55,9 @@ static void decode_stream(Job *j) {
 	/* E264_BENCH_LOOP_FILTER=<mode>: edge264_set_loop_filter on every decoder (tools/loop_filter_cost.py) */
 	const char *lf = getenv("E264_BENCH_LOOP_FILTER");
 	if (lf && atoi(lf) && (!edge264_set_loop_filter || edge264_set_loop_filter(dec, atoi(lf)))) { edge264_free(&dec); j->last_ret = -1; return; }
+	/* E264_BENCH_OUTPUT_LATENCY=<n>: edge264_set_output_latency on every decoder (tools/latency_cost.py) */
+	const char *ol = getenv("E264_BENCH_OUTPUT_LATENCY");
+	if (ol && *ol && (!edge264_set_output_latency || edge264_set_output_latency(dec, atoi(ol)))) { edge264_free(&dec); j->last_ret = -1; return; }
 	for (;;) {
 		const uint8_t *sc = nal < end ? edge264_find_start_code(nal, end, 0) : end;
 		long before = frames;

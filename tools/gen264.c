@@ -16,6 +16,13 @@
  *                                           include/edge264_loopfilter.h)
  *          [--density pct] [--qp Q] [--temporal] [--pcm permille] [--crop-bottom px] [--level idc]
  *          [--mvrange qpel] [--intra-pct P] [--skip-pct P]
+ *          [--no-vui]                       (no VUI in the SPS: the decoder infers max_num_reorder_frames and
+ *                                           max_dec_frame_buffering from the level, the case of many cameras)
+ *          [--reorder N]                    (max_num_reorder_frames N in the VUI bitstream_restriction, every other value
+ *                                           as without the option; with --no-vui, a VUI holding only bitstream_restriction
+ *                                           that states the values inferred from the level, with reorder N.  Every other
+ *                                           bit of the stream is the one written without the option: the twin of a decode
+ *                                           with edge264_set_output_latency(N), include/edge264_latency.h)
  *          [--crop-left px] [--crop-right px] [--crop-top px]   (even numbers; with --crop-bottom: frame cropping rectangle)
  *          [--direct4x4]                    (direct_8x8_inference_flag = 0: direct prediction per 4x4 block)
  *          [--nonref-p]                     (with --gop IP: some P pictures are not used for reference)
@@ -82,6 +89,7 @@ typedef struct GenState {
 	int cur_is_b;
 	int i_period;
 	int deblock_off;        /* --deblock-off: 0 none, 1 non-reference pictures, 2 all pictures */
+	int no_vui, reorder;    /* --no-vui; --reorder N (-1 without it) */
 	int direct4x4, nonref_p, extra_nals, bref, crop_left, crop_right, crop_top, mixed, ps_update, dpb_mode, mmco5, poc_type, max_long_idx_plus1, stat_rplm, stat_mmco[7], stat_idr_long;   /* --dpb: list modification + memory-management stress on I P P P streams; --poc-type 0|1|2 */
 	int wp_full, qp_walk, cqp_fixed, cqp[2], levels_big, pcm_extreme;   /* the standard's limits (file header) */
 } GenState;
@@ -121,6 +129,14 @@ static void put_scaling_matrix(GenState *g, BitWriter *w, int n_lists) {
 	}
 }
 
+/* MaxDpbFrames (A.3.1 h, Table A-1): what a decoder infers without bitstream_restriction */
+static int max_dpb_frames(int level, int mbs) {
+	const int max_dpb_mbs = level <= 10 || level == 9 ? 396 : level == 11 ? 900 : level <= 20 ? 2376 : level == 21 ? 4752 : level <= 30 ? 8100 :
+	                        level == 31 ? 18000 : level == 32 ? 20480 : level <= 41 ? 32768 : level == 42 ? 34816 : level == 50 ? 110400 :
+	                        level <= 52 ? 184320 : 696320;
+	return max_dpb_mbs / mbs < 16 ? max_dpb_mbs / mbs : 16;
+}
+
 /* subset: the subset SPS of --mvc (NAL unit 15, Stereo High, two views whose second predicts from the first) */
 static void write_sps(GenState *g, ByteBuf *out, int subset) {
 	BitWriter w; bw_init(&w, 4096);
@@ -141,12 +157,15 @@ static void write_sps(GenState *g, ByteBuf *out, int subset) {
 	const int any_crop = g->crop_bottom > 0 || g->crop_left > 0 || g->crop_right > 0 || g->crop_top > 0;
 	bw_u(&w, 1, any_crop);
 	if (any_crop) { bw_ue(&w, g->crop_left / 2); bw_ue(&w, g->crop_right / 2); bw_ue(&w, g->crop_top / 2); bw_ue(&w, g->crop_bottom / 2); }
-	bw_u(&w, 1, 1);                      /* vui_parameters_present_flag: only bitstream_restriction */
-	bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0);
-	bw_u(&w, 1, 1);
-	bw_u(&w, 1, 1); bw_ue(&w, 0); bw_ue(&w, 0); bw_ue(&w, 16); bw_ue(&w, 16);
-	bw_ue(&w, g->gop == 2 ? 1 : 0);     /* max_num_reorder_frames */
-	bw_ue(&w, g->refs + (g->gop == 2)); /* max_dec_frame_buffering */
+	const int vui = !g->no_vui || g->reorder >= 0;
+	bw_u(&w, 1, vui);                    /* vui_parameters_present_flag: only bitstream_restriction */
+	if (vui) {
+		bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0); bw_u(&w, 1, 0);
+		bw_u(&w, 1, 1);
+		bw_u(&w, 1, 1); bw_ue(&w, 0); bw_ue(&w, 0); bw_ue(&w, 16); bw_ue(&w, 16);
+		bw_ue(&w, g->reorder >= 0 ? g->reorder : g->gop == 2 ? 1 : 0);                      /* max_num_reorder_frames */
+		bw_ue(&w, g->no_vui ? max_dpb_frames(g->level, g->W * g->H) : g->refs + (g->gop == 2));   /* max_dec_frame_buffering */
+	}
 	if (subset) {
 		bw_u(&w, 1, 1);                      /* bit_equal_to_one */
 		bw_ue(&w, 1); bw_ue(&w, 0); bw_ue(&w, 1);   /* num_views_minus1, view_id 0 and 1 */
@@ -748,6 +767,8 @@ int main(int argc, char **argv) {
 	g->direct4x4 = argf(argc, argv, "--direct4x4"); g->nonref_p = argf(argc, argv, "--nonref-p"); g->extra_nals = argf(argc, argv, "--extra-nals");
 	g->bref = argf(argc, argv, "--bref");
 	g->i_period = argi(argc, argv, "--i-period", 0);
+	g->no_vui = argf(argc, argv, "--no-vui"); g->reorder = argi(argc, argv, "--reorder", -1);
+	if (g->reorder > 16) { fprintf(stderr, "gen264: --reorder takes 0..16\n"); return 2; }
 	for (int i = 1; i + 1 < argc; i++) if (!strcmp(argv[i], "--deblock-off")) {
 		g->deblock_off = !strcmp(argv[i + 1], "nonref") ? 1 : !strcmp(argv[i + 1], "all") ? 2 : -1;
 		if (g->deblock_off < 0) { fprintf(stderr, "gen264: --deblock-off takes nonref or all\n"); return 2; }
